@@ -6,6 +6,8 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <algorithm>
+
 #include "../../include/ptar.h"
 #include "ptar_generate.cuh"
 #include "ptar_gwb.cuh"
@@ -301,15 +303,20 @@ int launch_gen(const ptar_gen_params& p, cudaStream_t st) {
 template <bool INJECT, bool SLICE>
 int launch_mix(double* Zm, const double* M, const double* zin, int n_psr, int J, int64_t nreal, uint64_t seed, int64_t real0,
                int8_t* ZS, const double* zinv, int Jpad, int64_t rcap, cudaStream_t st, const char* what) {
-  const dim3 grid((J + ptar::MIX_JT - 1) / ptar::MIX_JT,
-                  static_cast<unsigned>((nreal + 4 * ptar::MX_GROUPS - 1) / (4 * ptar::MX_GROUPS)));
-  if (grid.y > 65535) return fail(-3, "ptar_gwb_mix: more than 262140 realizations per call%s");
   const int KP = (n_psr + 3) & ~3, NP = (n_psr + 7) & ~7;
   // draws [KP][132] + M [NP][KP + 4] doubles: 113 KB at 67 pulsars (2 CTAs per SM), the 227 KB limit is reached at 115 pulsars
   const size_t smem = sizeof(double) * (size_t(KP) * ptar::MX_ZS + size_t(NP) * (KP + 4));
   if (smem > 227 * 1024) return fail(-3, "ptar_gwb_mix: more than 115 pulsars do not fit the shared-memory tile%s");
   static SmemOptIn optin;   // per instantiation
   if (int rc = opt_in_smem(ptar::gwb_mix_dmma_kernel<INJECT, SLICE>, optin, 227 * 1024, what)) return rc;
+  // persistent: as many CTAs as are resident at once, each stages M once and loops over (column block, group) items
+  int dev = 0, n_sm = 0, per_sm = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e == cudaSuccess) e = cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, dev);
+  if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ptar::gwb_mix_dmma_kernel<INJECT, SLICE>, 256, smem);
+  if (e != cudaSuccess || per_sm < 1) return fail(-100, "ptar_gwb_mix: resident-CTA query: %s", cudaGetErrorString(e));
+  const int64_t items = int64_t((J + ptar::MIX_JT - 1) / ptar::MIX_JT) * ((nreal + 3) / 4);
+  const unsigned grid = static_cast<unsigned>(std::min<int64_t>(items, int64_t(n_sm) * per_sm));
   ptar::gwb_mix_dmma_kernel<INJECT, SLICE><<<grid, 256, smem, st>>>(Zm, M, zin, n_psr, J, nreal, ptar::philox_keys(seed), real0, ZS,
                                                                      zinv, Jpad, rcap);
   return check_launch(what);

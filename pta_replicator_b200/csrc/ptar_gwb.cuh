@@ -29,12 +29,14 @@ namespace ptar {
 
 // ---------------------------------------------------------------------------------------
 // ORF mixing: Zm[p][r][j] = sum_{q<=p} M[p][q] z[r][q][j]   (output pulsar-major).
-// Per CTA: 32 grid columns x up to MX_GROUPS Philox realization groups (4 realizations each), processed
-// one group at a time with M staged once in shared memory.  Per group: 128 rows (row = l*32 + jj),
-// D[row][p] = sum_q z[q][row] * M[p][q]; K = q padded to a multiple of 4, N = p padded to a multiple of
-// 8.  zs[q][row] has row stride 132 and ms[p][q] row stride KP+4 -> conflict-free 8x4 fragment gathers.
-// Warp w owns rows 16w..16w+15 (2 m-tiles) and all n-tiles; k-steps above the diagonal are skipped.
-constexpr int MIX_JT = 32, MX_ROWS = 128, MX_ZS = MX_ROWS + 4, MX_GROUPS = 1;
+// Persistent: each CTA stages the lower triangle of M once in shared memory, then loops over the work items
+// blockIdx.x, blockIdx.x + gridDim.x, ... = (32 grid columns, one Philox group of 4 realizations), the column
+// block fastest.  The grid is the resident-CTA count (2 per SM at 67 pulsars), so one CTA's draws run under the
+// other's MMAs.  Per item: 128 rows (row = l*32 + jj), D[row][p] = sum_q z[q][row] * M[p][q]; K = q padded to a
+// multiple of 4, N = p padded to a multiple of 8.  zs[q][row] has row stride 132 and ms[p][q] row stride KP+4 ->
+// conflict-free 8x4 fragment gathers.  Warp w owns rows 16w..16w+15 (2 m-tiles) and all n-tiles; k-steps above the
+// diagonal are skipped.
+constexpr int MIX_JT = 32, MX_ROWS = 128, MX_ZS = MX_ROWS + 4;
 
 // SLICE = true (throughput mode with the int8 tensor-core synthesis, n_psr <= 72): instead of fp64 Zm the kernel emits the
 // six signed radix-256 digit slices of Zm[p][r][j] / zscale[p] in the tensor core's K-major core-matrix tile layout
@@ -56,17 +58,20 @@ __global__ void __launch_bounds__(256, 2) gwb_mix_dmma_kernel(double* __restrict
   double* zs = mx_smem;                       // [KP][132]
   double* ms = mx_smem + size_t(KP) * MX_ZS;  // [NP][MS]
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int j0 = blockIdx.x * MIX_JT;
   for (int p = tid >> 5; p < NP; p += 8) {      // warp per row of M: no integer division by the run-time pitch
     for (int q = tid & 31; q < MS; q += 32) ms[p * MS + q] = (p < P && q <= p) ? __ldg(M + size_t(p) * P + q) : 0.0;
   }
   const int fr = lane >> 2, fk = lane & 3;
   const int row0 = warp * 16;
   const int n_nt = NP / 8;
-  for (int grp = 0; grp < MX_GROUPS; ++grp) {
-    const int64_t rbase = (int64_t(blockIdx.y) * MX_GROUPS + grp) * 4;
-    if (rbase >= nreal) break;
-    __syncthreads();  // previous group's fragments are consumed (and ms is visible)
+  const int n_jb = (J + MIX_JT - 1) / MIX_JT;
+  const int64_t n_items = int64_t(n_jb) * ((nreal + 3) / 4);
+  for (int64_t item = blockIdx.x; item < n_items; item += gridDim.x) {
+    const int j0 = static_cast<int>(item % n_jb) * MIX_JT;
+    const int64_t rbase = (item / n_jb) * 4;
+    __syncthreads();  // the previous item's draws and digits are consumed (and ms is visible)
+    // unrolled: independent Philox chains interleave (each thread draws ~9 of them per item, a long dependent chain each)
+#pragma unroll 3
     for (int idx = tid; idx < KP * MIX_JT; idx += 256) {
       const int q = idx / MIX_JT, jj = idx % MIX_JT, j = j0 + jj;
       double z[4] = {0, 0, 0, 0};
@@ -92,6 +97,7 @@ __global__ void __launch_bounds__(256, 2) gwb_mix_dmma_kernel(double* __restrict
       if (nt >= n_nt) break;
       double acc[2][2] = {{0.0, 0.0}, {0.0, 0.0}};
       const int kmax = min(KP, (nt * 8 + 8 + 3) & ~3);  // q <= p < nt*8+8
+#pragma unroll 4
       for (int k0 = 0; k0 < kmax; k0 += 4) {
         const double b = ms[(nt * 8 + fr) * MS + k0 + fk];
         const double a0 = zs[size_t(k0 + fk) * MX_ZS + row0 + fr];
