@@ -26,6 +26,8 @@
  *                          interp1d(ut, Res)(toas)                      red_noise.py:286-287
  *                          (+ CGW / deterministic delays)               deterministic.py:160-165
  *   ptar_philox_normals    np.random.randn (throughput-mode stream)     SURVEY.md 3.6
+ *   ptar_timing_project    the linear timing fit of SimulatedPulsar.fit simulate.py:44-69 (weighted least squares
+ *                          on a fixed design matrix; np.polyfit of add_burst(remove_quad) deterministic.py:777-779)
  */
 #ifndef PTAR_H
 #define PTAR_H
@@ -36,7 +38,10 @@
 extern "C" {
 #endif
 
-#define PTAR_VERSION 200  /* major*100 + minor; 2.0: column-major grid, g_ldr / c_rows, int8 GWB entry points, pshift phases */
+#define PTAR_VERSION 200  /* major*100 + minor; 2.0: column-major grid, g_ldr / c_rows, int8 GWB entry points, pshift phases.
+                             Later additions leave every 2.0 struct layout and entry point unchanged: the timing-model fit
+                             (ptar_timing_model, ptar_timing_project[_stage], ptar_run_job[_to_host]_tm) is new symbols only,
+                             so a caller detects it by looking the symbol up. */
 
 /* Geometry limits of the fused generator kernel. */
 #define PTAR_TILE_TOAS   1024  /* TOAs per tile (256 threads x 4)            */
@@ -224,6 +229,41 @@ int ptar_generate_stage(const ptar_gen_params* p, int stage, void* stream);
 int ptar_philox_normals(float* out, int kind, int psr, int64_t realization, int64_t idx0,
                         int64_t n, uint64_t seed, void* stream);
 
+/* Linear timing-model fit per pulsar (post-fit residuals).  For pulsar p with design matrix M_p (n_p x k_p) and
+ * per-TOA weights w = 1/sigma^2, the host factors the whitened matrix once, W^{1/2} M_p = Q_p R_p (thin QR, Q_p
+ * orthonormal columns), and the device applies
+ *     r' = r - W^{-1/2} Q_p (Q_p^T W^{1/2} r)
+ * to every realization row: the weighted least-squares residual r - M (M^T W M)^{-1} M^T W r without any k x k solve.
+ * Two kernels: the reduce kernel writes per (tile, realization) the k sums Q^T W^{1/2} r over the tile's TOAs
+ * (scratch partial[n_tiles][nreal][kmax]); the apply kernel adds a pulsar's tile partials in tile order and
+ * subtracts W^{-1/2} Q c.  Every sum runs in an order fixed by the tile and the TOA index only, so a post-fit row is
+ * bit-identical whatever nreal, chunking, real0 or launch grid produced it.  Only the n_p real TOAs of pulsars
+ * that have tiles are written; alignment slots and pulsars without a model are never touched. */
+#define PTAR_TM_KMAX 32   /* columns per pulsar */
+typedef struct {
+  int32_t n_psr;
+  int32_t n_tiles;          /* tiles of the pulsars that have a model                                      */
+  const ptar_tile* tiles;   /* [n_tiles]: toa_start, n_toa (<= PTAR_TILE_TOAS), toa_local0, psr are used; pulsar-
+                               major, tiles of one pulsar consecutive and in time order                      */
+  const int64_t* seg_off;   /* [n_psr] packed index of the pulsar's first TOA                               */
+  const int32_t* seg_len;   /* [n_psr] n_p, real TOAs of the pulsar                                         */
+  const int32_t* k;         /* [n_psr] k_p model columns (0: no model)                                      */
+  const int64_t* q_off;     /* [n_psr] offset of the pulsar's Q block: Q[q_off[p] + j * n_p + i], i local   */
+  const int32_t* tile0;     /* [n_psr] first tile of the pulsar in tiles[]                                  */
+  const int32_t* n_tile;    /* [n_psr] tiles of the pulsar                                                  */
+  const double* Q;          /* orthonormal columns of W^{1/2} M, engine (time-sorted) order                 */
+  const double* sqrtw;      /* [ld_out] 1/sigma per TOA on the packed axis                                  */
+  int32_t kmax;             /* max k_p (<= PTAR_TM_KMAX): row pitch of the partial sums                     */
+  int32_t reserved;
+} ptar_timing_model;
+
+/* out[r][ld_out], r < nreal, in place.  scratch: at least n_tiles * nreal * kmax doubles (device).
+ * ptar_timing_project_stage runs one of the two launches (stage 1 = reduce, 2 = apply) so a caller can time them. */
+int ptar_timing_project(double* out, int64_t ld_out, int32_t nreal, const ptar_timing_model* tm, double* scratch,
+                        int64_t scratch_len, void* stream);
+int ptar_timing_project_stage(double* out, int64_t ld_out, int32_t nreal, const ptar_timing_model* tm, double* scratch,
+                              int64_t scratch_len, int stage, void* stream);
+
 /* End-to-end job: GWB mix + synth + generate for realizations [real0, real0+nreal), then
  * (ptar_run_job_to_host) copy the residuals to pinned host memory, chunk by chunk, with the
  * copy of chunk c overlapping the generation of chunk c+1 on a second stream. */
@@ -268,6 +308,15 @@ int ptar_peer_copy(void* dst, const void* src, int64_t bytes, void* stream);
 int ptar_run_job(const ptar_job* job, int64_t real0, int32_t nreal, double* out, void* stream);
 int ptar_run_job_to_host(const ptar_job* job, int64_t real0, int64_t nreal, int32_t chunk,
                          double* out_host, double* dev_buf0, double* dev_buf1, void* stream0, void* stream1);
+
+/* The same two with the timing-model fit applied to every chunk right after ptar_generate (post-fit residuals);
+ * tm == NULL runs exactly ptar_run_job / ptar_run_job_to_host.  scratch: >= tm->n_tiles * chunk * tm->kmax doubles
+ * (chunk = nreal for ptar_run_job_tm). */
+int ptar_run_job_tm(const ptar_job* job, const ptar_timing_model* tm, double* scratch, int64_t scratch_len, int64_t real0,
+                    int32_t nreal, double* out, void* stream);
+int ptar_run_job_to_host_tm(const ptar_job* job, const ptar_timing_model* tm, double* scratch, int64_t scratch_len,
+                            int64_t real0, int64_t nreal, int32_t chunk, double* out_host, double* dev_buf0,
+                            double* dev_buf1, void* stream0, void* stream1);
 
 #ifdef __cplusplus
 }

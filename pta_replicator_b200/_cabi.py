@@ -19,11 +19,13 @@ TOA_ALIGN = 4
 I8_SLICES, I8_BM, I8_BN, I8_BK = 6, 128, 32, 32   # int8 wgmma GWB synthesis tile (csrc/ptar_gwb_i8.cuh)
 
 F_WHITE, F_ECORR, F_RED, F_GWB, F_DET, F_WHITE1 = 1, 2, 4, 8, 16, 32
+TM_KMAX = 32                                       # timing-model columns per pulsar (PTAR_TM_KMAX)
 K_WHITE1, K_WHITE2, K_ECORR, K_RED, K_GWB = 1, 2, 3, 4, 5
 
 EXPORTS = ("ptar_version", "ptar_last_error", "ptar_cholesky_lower", "ptar_fourier_basis", "ptar_cgw_delay", "ptar_cw_catalog", "ptar_burst_delay", "ptar_memory_delay",
            "ptar_gwb_mix", "ptar_gwb_synth", "ptar_gwb_mix_i8", "ptar_gwb_slice_i8", "ptar_gwb_synth_i8", "ptar_debug_i8_timestamps", "ptar_generate", "ptar_generate_stage", "ptar_philox_normals", "ptar_peer_export", "ptar_peer_open", "ptar_peer_close", "ptar_peer_copy", "ptar_run_job",
-           "ptar_run_job_to_host")
+           "ptar_run_job_to_host", "ptar_timing_project", "ptar_timing_project_stage",
+           "ptar_run_job_tm", "ptar_run_job_to_host_tm")
 
 
 class Tile(C.Structure):
@@ -55,6 +57,13 @@ class Job(C.Structure):
                 ("reserved", C.c_int32), ("Zm", C.c_void_p), ("Gbuf", C.c_void_p), ("gwb_zin", C.c_void_p),
                 ("AS", C.c_void_p), ("colscale", C.c_void_p), ("ZS", C.c_void_p), ("zscale", C.c_void_p), ("zinv", C.c_void_p),
                 ("tile_list_i8", C.c_void_p), ("rcap", C.c_int64), ("Jpad", C.c_int32), ("n_syn_tiles_i8", C.c_int32)]
+
+
+class TimingModel(C.Structure):
+    _fields_ = [("n_psr", C.c_int32), ("n_tiles", C.c_int32), ("tiles", C.c_void_p), ("seg_off", C.c_void_p),
+                ("seg_len", C.c_void_p), ("k", C.c_void_p), ("q_off", C.c_void_p), ("tile0", C.c_void_p),
+                ("n_tile", C.c_void_p), ("Q", C.c_void_p), ("sqrtw", C.c_void_p), ("kmax", C.c_int32),
+                ("reserved", C.c_int32)]
 
 
 _lib = None
@@ -97,6 +106,10 @@ def lib():
     L.ptar_peer_copy.argtypes = [vp, vp, i64, vp]
     L.ptar_run_job.argtypes = [C.POINTER(Job), i64, C.c_int32, vp, vp]
     L.ptar_run_job_to_host.argtypes = [C.POINTER(Job), i64, i64, C.c_int32, vp, vp, vp, vp, vp]
+    L.ptar_timing_project.argtypes = [vp, i64, C.c_int32, vp, vp, i64, vp]       # tm: address of a TimingModel
+    L.ptar_timing_project_stage.argtypes = [vp, i64, C.c_int32, vp, vp, i64, i32, vp]
+    L.ptar_run_job_tm.argtypes = [C.POINTER(Job), vp, vp, i64, i64, C.c_int32, vp, vp]
+    L.ptar_run_job_to_host_tm.argtypes = [C.POINTER(Job), vp, vp, i64, i64, i64, C.c_int32, vp, vp, vp, vp, vp]
     for name in EXPORTS:
         if name not in ("ptar_version", "ptar_last_error"):
             getattr(L, name).restype = C.c_int

@@ -13,6 +13,7 @@
 #include "ptar_gwb.cuh"
 #include "ptar_gwb_i8.cuh"
 #include "ptar_rng.cuh"
+#include "ptar_timing.cuh"
 
 namespace {
 
@@ -322,6 +323,21 @@ int launch_mix(double* Zm, const double* M, const double* zin, int n_psr, int J,
   return check_launch(what);
 }
 
+template <int KC>
+int launch_timing(double* out, int64_t ld, int32_t nreal, const ptar_timing_model& tm, double* scratch, int stage,
+                  cudaStream_t st) {
+  const dim3 grid(static_cast<unsigned>((nreal + ptar::tm_rb<KC>() - 1) / ptar::tm_rb<KC>()), static_cast<unsigned>(tm.n_tiles));
+  if (stage != 2) {
+    ptar::timing_reduce_kernel<KC><<<grid, ptar::TM_THREADS, 0, st>>>(out, ld, nreal, tm, scratch);
+    if (int rc = check_launch("ptar_timing_project (reduce)")) return rc;
+  }
+  if (stage != 1) {
+    ptar::timing_apply_kernel<KC><<<grid, ptar::TM_THREADS, 0, st>>>(out, ld, nreal, tm, scratch);
+    if (int rc = check_launch("ptar_timing_project (apply)")) return rc;
+  }
+  return 0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -584,7 +600,30 @@ int ptar_peer_copy(void* dst, const void* src, int64_t bytes, void* stream) {
   return 0;
 }
 
-int ptar_run_job(const ptar_job* job, int64_t real0, int32_t nreal, double* out, void* stream) {
+int ptar_timing_project_stage(double* out, int64_t ld_out, int32_t nreal, const ptar_timing_model* tm, double* scratch,
+                              int64_t scratch_len, int stage, void* stream) {
+  if (!out || !tm || nreal <= 0 || ld_out <= 0 || stage < 0 || stage > 2) return fail(-1, "ptar_timing_project: bad argument%s");
+  if (tm->n_tiles <= 0) return 0;   // no pulsar has a model
+  if (!tm->tiles || !tm->seg_len || !tm->k || !tm->q_off || !tm->tile0 || !tm->n_tile || !tm->Q || !tm->sqrtw || !scratch)
+    return fail(-2, "ptar_timing_project: model arrays / scratch missing%s");
+  if (tm->kmax <= 0 || tm->kmax > PTAR_TM_KMAX) return fail(-2, "ptar_timing_project: kmax must be in 1..32%s");
+  if (tm->n_tiles > 65535) return fail(-3, "ptar_timing_project: more than 65535 tiles%s");
+  if (scratch_len < int64_t(tm->n_tiles) * nreal * tm->kmax)
+    return fail(-2, "ptar_timing_project: scratch too small (need n_tiles * nreal * kmax doubles)%s");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (tm->kmax <= 4) return launch_timing<4>(out, ld_out, nreal, *tm, scratch, stage, st);
+  if (tm->kmax <= 8) return launch_timing<8>(out, ld_out, nreal, *tm, scratch, stage, st);
+  if (tm->kmax <= 16) return launch_timing<16>(out, ld_out, nreal, *tm, scratch, stage, st);
+  return launch_timing<32>(out, ld_out, nreal, *tm, scratch, stage, st);
+}
+
+int ptar_timing_project(double* out, int64_t ld_out, int32_t nreal, const ptar_timing_model* tm, double* scratch,
+                        int64_t scratch_len, void* stream) {
+  return ptar_timing_project_stage(out, ld_out, nreal, tm, scratch, scratch_len, 0, stream);
+}
+
+int ptar_run_job_tm(const ptar_job* job, const ptar_timing_model* tm, double* scratch, int64_t scratch_len, int64_t real0,
+                    int32_t nreal, double* out, void* stream) {
   if (!job || !out || nreal <= 0) return fail(-1, "ptar_run_job: bad argument%s");
   ptar_gen_params g = job->gen;
   g.real0 = real0;
@@ -618,11 +657,18 @@ int ptar_run_job(const ptar_job* job, int64_t real0, int32_t nreal, double* out,
     if (rc) return rc;
     g.G = job->Gbuf;
   }
-  return ptar_generate(&g, stream);
+  if (int rc = ptar_generate(&g, stream)) return rc;
+  if (tm) return ptar_timing_project(out, g.ld_out, nreal, tm, scratch, scratch_len, stream);
+  return 0;
 }
 
-int ptar_run_job_to_host(const ptar_job* job, int64_t real0, int64_t nreal, int32_t chunk, double* out_host,
-                         double* dev_buf0, double* dev_buf1, void* stream0, void* stream1) {
+int ptar_run_job(const ptar_job* job, int64_t real0, int32_t nreal, double* out, void* stream) {
+  return ptar_run_job_tm(job, nullptr, nullptr, 0, real0, nreal, out, stream);
+}
+
+int ptar_run_job_to_host_tm(const ptar_job* job, const ptar_timing_model* tm, double* scratch, int64_t scratch_len,
+                            int64_t real0, int64_t nreal, int32_t chunk, double* out_host, double* dev_buf0,
+                            double* dev_buf1, void* stream0, void* stream1) {
   if (!job || !out_host || !dev_buf0 || !dev_buf1 || chunk <= 0 || (chunk & 3) || nreal <= 0)
     return fail(-1, "ptar_run_job_to_host: bad argument (chunk must be a positive multiple of 4)%s");
   cudaStream_t s0 = static_cast<cudaStream_t>(stream0), s1 = static_cast<cudaStream_t>(stream1);
@@ -650,7 +696,7 @@ int ptar_run_job_to_host(const ptar_job* job, int64_t real0, int64_t nreal, int3
     if (j.gen.zb) j.gen.zb += done * j.gen.n_bucket_total;
     if (j.gen.zrn) j.gen.zrn += done * int64_t(j.gen.n_psr) * j.gen.J;
     if (j.gwb_zin) j.gwb_zin += done * int64_t(j.gen.n_psr) * j.Jg;
-    rc = ptar_run_job(&j, real0 + done, n, bufs[b], s0);
+    rc = ptar_run_job_tm(&j, tm, scratch, scratch_len, real0 + done, n, bufs[b], s0);
     if (rc) break;
     if (!ok(cudaEventRecord(gen_done[b], s0)) || !ok(cudaStreamWaitEvent(s1, gen_done[b], 0))) break;
     if (!ok(cudaMemcpyAsync(out_host + done * ld, bufs[b], sizeof(double) * size_t(n) * ld, cudaMemcpyDeviceToHost, s1))) break;
@@ -669,6 +715,11 @@ int ptar_run_job_to_host(const ptar_job* job, int64_t real0, int64_t nreal, int3
   ok(cudaGetLastError());
   if (e != cudaSuccess) return fail(-100, "ptar_run_job_to_host: %s", cudaGetErrorString(e));
   return 0;
+}
+
+int ptar_run_job_to_host(const ptar_job* job, int64_t real0, int64_t nreal, int32_t chunk, double* out_host,
+                         double* dev_buf0, double* dev_buf1, void* stream0, void* stream1) {
+  return ptar_run_job_to_host_tm(job, nullptr, nullptr, 0, real0, nreal, chunk, out_host, dev_buf0, dev_buf1, stream0, stream1);
 }
 
 }  // extern "C"
