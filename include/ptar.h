@@ -28,6 +28,8 @@
  *   ptar_philox_normals    np.random.randn (throughput-mode stream)     SURVEY.md 3.6
  *   ptar_timing_project    the linear timing fit of SimulatedPulsar.fit simulate.py:44-69 (weighted least squares
  *                          on a fixed design matrix; np.polyfit of add_burst(remove_quad) deterministic.py:777-779)
+ *   ptar_os_project /      no counterpart: the frequentist optimal statistic of the realizations, reduced on the
+ *   ptar_os_pairs          device instead of gathering the rows
  */
 #ifndef PTAR_H
 #define PTAR_H
@@ -40,8 +42,9 @@ extern "C" {
 
 #define PTAR_VERSION 200  /* major*100 + minor; 2.0: column-major grid, g_ldr / c_rows, int8 GWB entry points, pshift phases.
                              Later additions leave every 2.0 struct layout and entry point unchanged: the timing-model fit
-                             (ptar_timing_model, ptar_timing_project[_stage], ptar_run_job[_to_host]_tm) is new symbols only,
-                             so a caller detects it by looking the symbol up. */
+                             (ptar_timing_model, ptar_timing_project[_stage], ptar_run_job[_to_host]_tm) and the optimal
+                             statistic (ptar_os_model, ptar_os_project[_stage], ptar_os_pairs) are new symbols only, so a
+                             caller detects them by looking the symbol up. */
 
 /* Geometry limits of the fused generator kernel. */
 #define PTAR_TILE_TOAS   1024  /* TOAs per tile (256 threads x 4)            */
@@ -263,6 +266,53 @@ int ptar_timing_project(double* out, int64_t ld_out, int32_t nreal, const ptar_t
                         int64_t scratch_len, void* stream);
 int ptar_timing_project_stage(double* out, int64_t ld_out, int32_t nreal, const ptar_timing_model* tm, double* scratch,
                               int64_t scratch_len, int stage, void* stream);
+
+/* Optimal statistic (csrc/ptar_os.cuh).  The host derives, once per recipe, C_a = P_a^{-1} F_gw,a for every pulsar
+ * (P_a the noise covariance with the timing model marginalised, F_gw,a the 2K sin/cos columns of the GW basis), the
+ * pair normalisations t_ab = tr(Z_a phi~ Z_b phi~) with Z_a = F_gw,a^T C_a, the template weights Gamma^o_ab and the
+ * inverse F^{-1} of the multiple-component Fisher matrix.  Per realization r:
+ *   ptar_os_project  X[r][p][j] = sum_i C[i][j] rows[r][i] over the TOAs i of pulsar p.  Two launches: a tile GEMM on
+ *                    the fp64 tensor cores (partial[n_tiles][nreal][ncp]) and the sum of each pulsar's tile partials
+ *                    in tile order.  rows: ld % 4 == 0, 32-byte aligned; alignment slots of the packed axis are ignored.
+ *   ptar_os_pairs    x_p = X[r][p] phi~^{1/2};  d_ab = x_a . x_b (a < b, the order of `pairs`);
+ *                    rho[r][q] = d_ab / t_ab (rho may be NULL);  b_o = sum_q orf[o][q] d_q;
+ *                    a2[r][o] = b_o / dnorm[o];  snr[r][o] = b_o / dsqrt[o];  a2_mc[r][o] = sum_o' finv[o][o'] b_o'.
+ * Every sum runs in an order fixed by the tile, the TOA index and the pair list only: outputs are bit-identical
+ * whatever nreal, chunking, real0 or launch grid produced the rows.  ptar_os_project_stage runs one of the two
+ * launches of ptar_os_project (stage 1 = tile GEMM, 2 = tile sums) so a caller can time them. */
+#define PTAR_OS_MAX_NC  32    /* GW-basis columns (2K)                 */
+#define PTAR_OS_MAX_ORF 4     /* templates                             */
+#define PTAR_OS_MAX_PSR 256   /* pulsars (pair kernel: x in shared memory) */
+typedef struct {
+  int32_t n_psr;
+  int32_t n_tiles;
+  const ptar_tile* tiles;   /* [n_tiles]: toa_start, n_toa (<= PTAR_TILE_TOAS), psr are used; tiles of one pulsar
+                               consecutive and in time order                                                    */
+  const int32_t* tile0;     /* [n_psr] first tile of the pulsar                                                 */
+  const int32_t* n_tile;    /* [n_psr] tiles of the pulsar                                                      */
+  const double* C;          /* [ld][ncp] row i = C_a[i][0..nc) of the TOA's pulsar, zero in columns >= nc and in
+                               alignment slots                                                                  */
+  int32_t nc;               /* 2K <= PTAR_OS_MAX_NC                                                             */
+  int32_t ncp;              /* nc rounded up to a multiple of 8                                                 */
+  const double* sqrt_phi;   /* [ncp] phi~^{1/2} per column                                                      */
+  int32_t n_pairs;
+  int32_t n_orf;            /* <= PTAR_OS_MAX_ORF                                                               */
+  const int32_t* pairs;     /* [n_pairs][2] (a, b), a < b                                                       */
+  const double* t_ab;       /* [n_pairs]                                                                        */
+  const double* orf;        /* [n_orf][n_pairs] Gamma^o_ab                                                      */
+  const double* dnorm;      /* [n_orf] D_o = sum_q Gamma^o_q^2 t_q                                              */
+  const double* dsqrt;      /* [n_orf] sqrt(D_o)                                                                */
+  const double* finv;       /* [n_orf][n_orf] F^{-1}, F_oo' = sum_q Gamma^o_q Gamma^o'_q t_q                    */
+} ptar_os_model;
+
+/* partial: >= n_tiles * nreal * ncp doubles; X: [nreal][n_psr][ncp]. */
+int ptar_os_project(const double* rows, int64_t ld, int32_t nreal, const ptar_os_model* os, double* partial,
+                    int64_t partial_len, double* X, void* stream);
+int ptar_os_project_stage(const double* rows, int64_t ld, int32_t nreal, const ptar_os_model* os, double* partial,
+                          int64_t partial_len, double* X, int stage, void* stream);
+/* rho: [nreal][n_pairs] or NULL; a2, snr, a2_mc: [nreal][n_orf]. */
+int ptar_os_pairs(const double* X, int32_t nreal, const ptar_os_model* os, double* rho, double* a2, double* snr,
+                  double* a2_mc, void* stream);
 
 /* End-to-end job: GWB mix + synth + generate for realizations [real0, real0+nreal), then
  * (ptar_run_job_to_host) copy the residuals to pinned host memory, chunk by chunk, with the

@@ -12,6 +12,7 @@
 #include "ptar_generate.cuh"
 #include "ptar_gwb.cuh"
 #include "ptar_gwb_i8.cuh"
+#include "ptar_os.cuh"
 #include "ptar_rng.cuh"
 #include "ptar_timing.cuh"
 
@@ -620,6 +621,72 @@ int ptar_timing_project_stage(double* out, int64_t ld_out, int32_t nreal, const 
 int ptar_timing_project(double* out, int64_t ld_out, int32_t nreal, const ptar_timing_model* tm, double* scratch,
                         int64_t scratch_len, void* stream) {
   return ptar_timing_project_stage(out, ld_out, nreal, tm, scratch, scratch_len, 0, stream);
+}
+
+int ptar_os_project_stage(const double* rows, int64_t ld, int32_t nreal, const ptar_os_model* os, double* partial,
+                          int64_t partial_len, double* X, int stage, void* stream) {
+  if (!rows || !os || !partial || !X || nreal <= 0 || ld <= 0 || stage < 0 || stage > 2)
+    return fail(-1, "ptar_os_project: bad argument%s");
+  if (!os->tiles || !os->tile0 || !os->n_tile || !os->C || os->n_tiles <= 0 || os->n_psr <= 0)
+    return fail(-2, "ptar_os_project: model arrays missing%s");
+  if (os->nc <= 0 || os->nc > PTAR_OS_MAX_NC || os->ncp != ((os->nc + 7) & ~7))
+    return fail(-2, "ptar_os_project: need 0 < nc <= 32 and ncp = nc rounded up to a multiple of 8%s");
+  if ((ld & 3) || (reinterpret_cast<uintptr_t>(rows) & 31))
+    return fail(-2, "ptar_os_project: rows must be 32-byte aligned with ld %% 4 == 0%s");
+  if (os->n_tiles > 65535) return fail(-3, "ptar_os_project: more than 65535 tiles%s");
+  if (partial_len < int64_t(os->n_tiles) * nreal * os->ncp)
+    return fail(-2, "ptar_os_project: partial too small (need n_tiles * nreal * ncp doubles)%s");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (stage != 2) {
+    const dim3 grid(static_cast<unsigned>((nreal + ptar::OS_RB - 1) / ptar::OS_RB), static_cast<unsigned>(os->n_tiles));
+    const int nt = os->ncp / 8;
+    static SmemOptIn optin[4];
+    switch (nt) {
+#define PTAR_OS_LAUNCH(NT)                                                                                          \
+  case NT:                                                                                                          \
+    if (int rc = opt_in_smem(ptar::os_project_kernel<NT>, optin[NT - 1], ptar::OS_SMEM, "ptar_os_project")) return rc; \
+    ptar::os_project_kernel<NT><<<grid, ptar::OS_THREADS, ptar::OS_SMEM, st>>>(rows, ld, nreal, *os, partial);      \
+    break;
+      PTAR_OS_LAUNCH(1)
+      PTAR_OS_LAUNCH(2)
+      PTAR_OS_LAUNCH(3)
+      PTAR_OS_LAUNCH(4)
+#undef PTAR_OS_LAUNCH
+    }
+    if (int rc = check_launch("ptar_os_project (tile GEMM)")) return rc;
+  }
+  if (stage != 1) {
+    const int64_t total = int64_t(nreal) * os->n_psr * os->ncp;
+    ptar::os_sum_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(partial, nreal, *os, X);
+    if (int rc = check_launch("ptar_os_project (tile sums)")) return rc;
+  }
+  return 0;
+}
+
+int ptar_os_project(const double* rows, int64_t ld, int32_t nreal, const ptar_os_model* os, double* partial,
+                    int64_t partial_len, double* X, void* stream) {
+  return ptar_os_project_stage(rows, ld, nreal, os, partial, partial_len, X, 0, stream);
+}
+
+int ptar_os_pairs(const double* X, int32_t nreal, const ptar_os_model* os, double* rho, double* a2, double* snr,
+                  double* a2_mc, void* stream) {
+  if (!X || !os || !a2 || !snr || !a2_mc || nreal <= 0) return fail(-1, "ptar_os_pairs: bad argument%s");
+  if (!os->sqrt_phi || !os->pairs || !os->t_ab || !os->orf || !os->dnorm || !os->dsqrt || !os->finv)
+    return fail(-2, "ptar_os_pairs: model arrays missing%s");
+  if (os->n_psr < 2 || os->n_psr > PTAR_OS_MAX_PSR) return fail(-3, "ptar_os_pairs: need 2..256 pulsars%s");
+  if (os->n_orf <= 0 || os->n_orf > PTAR_OS_MAX_ORF || os->n_pairs <= 0)
+    return fail(-2, "ptar_os_pairs: need 1..4 templates and at least one pair%s");
+  if (os->nc <= 0 || os->nc > PTAR_OS_MAX_NC || os->ncp != ((os->nc + 7) & ~7))
+    return fail(-2, "ptar_os_pairs: need 0 < nc <= 32 and ncp = nc rounded up to a multiple of 8%s");
+  const size_t smem = sizeof(double) * (size_t(os->n_psr) * os->ncp + size_t(PTAR_OS_MAX_ORF) * ptar::OS_PAIR_THREADS);
+  static SmemOptIn optin;
+  if (int rc = opt_in_smem(ptar::os_pairs_kernel, optin, sizeof(double) * (size_t(PTAR_OS_MAX_PSR) * PTAR_OS_MAX_NC +
+                                                                           size_t(PTAR_OS_MAX_ORF) * ptar::OS_PAIR_THREADS),
+                           "ptar_os_pairs"))
+    return rc;
+  ptar::os_pairs_kernel<<<static_cast<unsigned>(nreal), ptar::OS_PAIR_THREADS, smem, static_cast<cudaStream_t>(stream)>>>(
+      X, nreal, *os, rho, a2, snr, a2_mc);
+  return check_launch("ptar_os_pairs");
 }
 
 int ptar_run_job_tm(const ptar_job* job, const ptar_timing_model* tm, double* scratch, int64_t scratch_len, int64_t real0,
