@@ -12,6 +12,12 @@ achieved bandwidth of the tile GEMM at the algorithmic 8 B per output (one fp64 
 realization) and its fraction of the data-sheet 3.35 TB/s; ``setup_s`` = batch + recipe + plan + compile, of which
 ``os_statics_s`` is the optimal statistic's host statics.  The card name and power limit are read with a read-only
 nvidia-smi query in the same run.  Writes nothing into the tree.
+
+    python bench_os.py --null {phase_shift,sky_scramble} [--n-null N]
+
+adds ``set_os_null(method, n=N)`` (default 1024; HD template) to the same workload: the step then also returns each
+realization's null count and p-value, and the line gains ``os_null``: the GEMM's achieved TFLOP/s at the algorithmic
+2 R (N + 1) Kd flop against the data-sheet 67 TFLOP/s of fp64 tensor cores, V's bytes and the null statics' host time.
 """
 from __future__ import annotations
 
@@ -36,6 +42,8 @@ def main():
     ap.add_argument("--nreal", type=int, default=1000)
     ap.add_argument("--kind", default="full", choices=["full", "epoch"])
     ap.add_argument("--taylor-tol", type=float, default=1e-13)
+    ap.add_argument("--null", default=None, choices=["phase_shift", "sky_scramble"])
+    ap.add_argument("--n-null", type=int, default=1024)
     args = ap.parse_args()
     args.split, args.chunk, args.rc = False, 0, 0
 
@@ -50,6 +58,8 @@ def main():
     for i in range(b.n_psr):
         b.set_timing_model(i, poly=2, jumps="f")
     b.set_optimal_statistic()
+    if args.null:
+        b.set_os_null(args.null, n=args.n_null)
     b.compile()
     setup_s = time.perf_counter() - t0
     R = args.nreal
@@ -87,6 +97,17 @@ def main():
                            "algorithmic_bytes_per_output": 8, "algorithmic_GBps": gbps, "frac": gbps / hbm, "peak": hbm,
                            "peak_source": how},
             "setup_s": setup_s, "os_statics_s": st["setup_s"], "card": card()}
+    if args.null:
+        nl = st["null"]
+        kd, ncol = int(nl["model"].kd), nl["n_col"]
+        tflops = 2.0 * R * ncol * kd / (kms["os_null_gemm"] * 1e-3) / 1e12
+        line["metric"] = line["metric"].replace("optimal_statistic", f"optimal_statistic + {args.null} null")
+        line["workload"] += f" + {args.null} null of the HD S/N ({args.n_null} columns + the template, Kd = {kd})"
+        line["os_null"] = {"method": args.null, "n": args.n_null, "kd": kd, "kernel": "os_null_gemm_kernel (DMMA)",
+                           "gemm_ms_per_step": kms["os_null_gemm"], "gemm_flop": 2.0 * R * ncol * kd,
+                           "gemm_TFLOPs": tflops, "frac_of_67_TFLOPs": tflops / 67.0,
+                           "V_bytes": int(nl["dev"]["V"].numel()) * 8, "U_bytes_per_chunk": int(b._os_null_U.numel()) * 8,
+                           "null_statics_s": nl["setup_s"]}
     print(json.dumps(line), flush=True)
 
 

@@ -30,6 +30,7 @@
  *                          on a fixed design matrix; np.polyfit of add_burst(remove_quad) deterministic.py:777-779)
  *   ptar_os_project /      no counterpart: the frequentist optimal statistic of the realizations, reduced on the
  *   ptar_os_pairs          device instead of gathering the rows
+ *   ptar_os_null           no counterpart: phase-shift / sky-scramble null distribution and p-value per realization
  */
 #ifndef PTAR_H
 #define PTAR_H
@@ -43,8 +44,9 @@ extern "C" {
 #define PTAR_VERSION 200  /* major*100 + minor; 2.0: column-major grid, g_ldr / c_rows, int8 GWB entry points, pshift phases.
                              Later additions leave every 2.0 struct layout and entry point unchanged: the timing-model fit
                              (ptar_timing_model, ptar_timing_project[_stage], ptar_run_job[_to_host]_tm) and the optimal
-                             statistic (ptar_os_model, ptar_os_project[_stage], ptar_os_pairs) are new symbols only, so a
-                             caller detects them by looking the symbol up. */
+                             statistic (ptar_os_model, ptar_os_project[_stage], ptar_os_pairs) and its null distributions
+                             (ptar_os_null_model, ptar_os_null[_stage]) are new symbols only, so a caller detects them by
+                             looking the symbol up. */
 
 /* Geometry limits of the fused generator kernel. */
 #define PTAR_TILE_TOAS   1024  /* TOAs per tile (256 threads x 4)            */
@@ -313,6 +315,39 @@ int ptar_os_project_stage(const double* rows, int64_t ld, int32_t nreal, const p
 /* rho: [nreal][n_pairs] or NULL; a2, snr, a2_mc: [nreal][n_orf]. */
 int ptar_os_pairs(const double* X, int32_t nreal, const ptar_os_model* os, double* rho, double* a2, double* snr,
                   double* a2_mc, void* stream);
+
+/* Null distribution of one template's S/N (csrc/ptar_os_null.cuh): phase shifts or sky scrambles, drawn once on the
+ * host and shared by every realization.  Columns s = 0..n_col-1: column 0 is the unshifted, unscrambled template,
+ * columns 1.. the null set.  Per realization r, from the X of ptar_os_project and x = X phi~^{1/2}:
+ *   S/N[r][s] = (sum_kd U[r][kd] V[kd][s]) / dsqrt[s]
+ *     PTAR_OS_NULL_PHASE_SHIFT   kd = (q, k, c), kd = 2 (q K + k) + c, K = nc / 2, q = (a, b) the pairs of os:
+ *                                U[(q,k,0)] = x_a,2k x_b,2k + x_a,2k+1 x_b,2k+1;  U[(q,k,1)] = x_a,2k+1 x_b,2k - x_a,2k x_b,2k+1
+ *                                V[(q,k,0)][s] = Gamma_q cos(phi_s,a,k - phi_s,b,k);  V[(q,k,1)][s] = Gamma_q sin(...)
+ *     PTAR_OS_NULL_SKY_SCRAMBLE  kd = q:  U[q] = x_a . x_b;  V[q][s] = Gamma^s_q (the template at scrambled positions)
+ *   exceed[r] = #{s >= 1 : S/N[r][s] >= S/N[r][0]};  fap[r] = (1 + exceed[r]) / n_col.
+ * Three launches: prepare (U, zero past kd), the GEMM on the fp64 tensor cores, count.  Each output is summed in an
+ * order fixed by kd only: outputs are bit-identical whatever nreal, chunking or real0.  ptar_os_null_stage runs one
+ * launch (stage 1 = prepare, 2 = GEMM, 3 = count; 0 = all three) so a caller can time them. */
+#define PTAR_OS_MAX_NULL 65536          /* null columns (n_col - 1) */
+#define PTAR_OS_NULL_PHASE_SHIFT  1
+#define PTAR_OS_NULL_SKY_SCRAMBLE 2
+typedef struct {
+  int32_t method;           /* PTAR_OS_NULL_PHASE_SHIFT or PTAR_OS_NULL_SKY_SCRAMBLE                             */
+  int32_t n_col;            /* columns: 2 .. PTAR_OS_MAX_NULL + 1                                                */
+  int32_t n_colp;           /* n_col rounded up to a multiple of 64                                              */
+  int32_t reserved;
+  int64_t kd;               /* 2 K n_pairs (phase shift) or n_pairs (sky scramble)                               */
+  int64_t kdp;              /* kd rounded up to a multiple of 32                                                 */
+  const double* V;          /* [n_colp][kdp]: V^T, row s = column s of V, zero past kd and in rows >= n_col      */
+  const double* dsqrt;      /* [n_col] sqrt(D_s)                                                                 */
+} ptar_os_null_model;
+
+/* U: scratch of nreal * kdp doubles; snr: [nreal][n_col]; exceed: [nreal] int64; fap: [nreal].  X and os as for
+ * ptar_os_pairs. */
+int ptar_os_null(const double* X, int32_t nreal, const ptar_os_model* os, const ptar_os_null_model* null_model,
+                 double* U, double* snr, int64_t* exceed, double* fap, void* stream);
+int ptar_os_null_stage(const double* X, int32_t nreal, const ptar_os_model* os, const ptar_os_null_model* null_model,
+                       double* U, double* snr, int64_t* exceed, double* fap, int stage, void* stream);
 
 /* End-to-end job: GWB mix + synth + generate for realizations [real0, real0+nreal), then
  * (ptar_run_job_to_host) copy the residuals to pinned host memory, chunk by chunk, with the

@@ -25,8 +25,12 @@ K_WHITE1, K_WHITE2, K_ECORR, K_RED, K_GWB = 1, 2, 3, 4, 5
 EXPORTS = ("ptar_version", "ptar_last_error", "ptar_cholesky_lower", "ptar_fourier_basis", "ptar_cgw_delay", "ptar_cw_catalog", "ptar_burst_delay", "ptar_memory_delay",
            "ptar_gwb_mix", "ptar_gwb_synth", "ptar_gwb_mix_i8", "ptar_gwb_slice_i8", "ptar_gwb_synth_i8", "ptar_debug_i8_timestamps", "ptar_generate", "ptar_generate_stage", "ptar_philox_normals", "ptar_peer_export", "ptar_peer_open", "ptar_peer_close", "ptar_peer_copy", "ptar_run_job",
            "ptar_run_job_to_host", "ptar_timing_project", "ptar_timing_project_stage",
-           "ptar_run_job_tm", "ptar_run_job_to_host_tm", "ptar_os_project", "ptar_os_project_stage", "ptar_os_pairs")
+           "ptar_run_job_tm", "ptar_run_job_to_host_tm", "ptar_os_project", "ptar_os_project_stage", "ptar_os_pairs",
+           "ptar_os_null", "ptar_os_null_stage")
 OS_MAX_NC, OS_MAX_ORF, OS_MAX_PSR = 32, 4, 256     # optimal statistic: GW-basis columns, templates, pulsars (ptar.h)
+OS_MAX_NULL = 65536                                # null columns of ptar_os_null (PTAR_OS_MAX_NULL)
+OS_NULL_PHASE_SHIFT, OS_NULL_SKY_SCRAMBLE = 1, 2
+OS_NULL_BK, OS_NULL_BN = 32, 64                    # kd / column padding of ptar_os_null_model (csrc/ptar_os_null.cuh)
 
 
 class Tile(C.Structure):
@@ -72,6 +76,11 @@ class OsModel(C.Structure):
                 ("n_tile", C.c_void_p), ("C", C.c_void_p), ("nc", C.c_int32), ("ncp", C.c_int32), ("sqrt_phi", C.c_void_p),
                 ("n_pairs", C.c_int32), ("n_orf", C.c_int32), ("pairs", C.c_void_p), ("t_ab", C.c_void_p),
                 ("orf", C.c_void_p), ("dnorm", C.c_void_p), ("dsqrt", C.c_void_p), ("finv", C.c_void_p)]
+
+
+class OsNullModel(C.Structure):
+    _fields_ = [("method", C.c_int32), ("n_col", C.c_int32), ("n_colp", C.c_int32), ("reserved", C.c_int32),
+                ("kd", C.c_int64), ("kdp", C.c_int64), ("V", C.c_void_p), ("dsqrt", C.c_void_p)]
 
 
 _lib = None
@@ -121,6 +130,8 @@ def lib():
     L.ptar_os_project.argtypes = [vp, i64, C.c_int32, vp, vp, i64, vp, vp]            # os: address of an OsModel
     L.ptar_os_project_stage.argtypes = [vp, i64, C.c_int32, vp, vp, i64, vp, i32, vp]
     L.ptar_os_pairs.argtypes = [vp, C.c_int32, vp, vp, vp, vp, vp, vp]
+    L.ptar_os_null.argtypes = [vp, C.c_int32, vp, vp, vp, vp, vp, vp, vp]                # null: address of an OsNullModel
+    L.ptar_os_null_stage.argtypes = [vp, C.c_int32, vp, vp, vp, vp, vp, vp, i32, vp]
     for name in EXPORTS:
         if name not in ("ptar_version", "ptar_last_error"):
             getattr(L, name).restype = C.c_int

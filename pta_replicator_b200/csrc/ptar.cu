@@ -13,6 +13,7 @@
 #include "ptar_gwb.cuh"
 #include "ptar_gwb_i8.cuh"
 #include "ptar_os.cuh"
+#include "ptar_os_null.cuh"
 #include "ptar_rng.cuh"
 #include "ptar_timing.cuh"
 
@@ -687,6 +688,51 @@ int ptar_os_pairs(const double* X, int32_t nreal, const ptar_os_model* os, doubl
   ptar::os_pairs_kernel<<<static_cast<unsigned>(nreal), ptar::OS_PAIR_THREADS, smem, static_cast<cudaStream_t>(stream)>>>(
       X, nreal, *os, rho, a2, snr, a2_mc);
   return check_launch("ptar_os_pairs");
+}
+
+int ptar_os_null_stage(const double* X, int32_t nreal, const ptar_os_model* os, const ptar_os_null_model* nl, double* U,
+                       double* snr, int64_t* exceed, double* fap, int stage, void* stream) {
+  if (!X || !os || !nl || !U || !snr || !exceed || !fap || nreal <= 0 || stage < 0 || stage > 3)
+    return fail(-1, "ptar_os_null: bad argument%s");
+  if (!os->sqrt_phi || !os->pairs || !nl->V || !nl->dsqrt) return fail(-2, "ptar_os_null: model arrays missing%s");
+  if (os->n_psr < 2 || os->n_psr > PTAR_OS_MAX_PSR || os->n_pairs != os->n_psr * (os->n_psr - 1) / 2)
+    return fail(-3, "ptar_os_null: need 2..256 pulsars and every pair%s");
+  if (os->nc <= 0 || os->nc > PTAR_OS_MAX_NC || (os->nc & 1) || os->ncp != ((os->nc + 7) & ~7))
+    return fail(-2, "ptar_os_null: need an even 0 < nc <= 32 and ncp = nc rounded up to a multiple of 8%s");
+  if (nl->method != PTAR_OS_NULL_PHASE_SHIFT && nl->method != PTAR_OS_NULL_SKY_SCRAMBLE)
+    return fail(-2, "ptar_os_null: unknown method%s");
+  if (nl->n_col < 2 || nl->n_col > PTAR_OS_MAX_NULL + 1 || nl->n_colp != ((nl->n_col + ptar::NL_BN - 1) & ~(ptar::NL_BN - 1)))
+    return fail(-2, "ptar_os_null: need 2 <= n_col <= 65537 and n_colp = n_col rounded up to a multiple of 64%s");
+  const int64_t kd = nl->method == PTAR_OS_NULL_PHASE_SHIFT ? int64_t(os->n_pairs) * os->nc : int64_t(os->n_pairs);
+  if (nl->kd != kd || nl->kdp != ((kd + ptar::NL_BK - 1) & ~int64_t(ptar::NL_BK - 1)))
+    return fail(-2, "ptar_os_null: kd must be 2 K n_pairs (phase shift) or n_pairs (sky scramble), kdp kd rounded up to 32%s");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (stage == 0 || stage == 1) {
+    const size_t smem = sizeof(double) * size_t(os->n_psr) * os->ncp;
+    static SmemOptIn optin;
+    if (int rc = opt_in_smem(ptar::os_null_prepare_kernel, optin, sizeof(double) * size_t(PTAR_OS_MAX_PSR) * PTAR_OS_MAX_NC,
+                             "ptar_os_null (prepare)"))
+      return rc;
+    ptar::os_null_prepare_kernel<<<static_cast<unsigned>(nreal), ptar::NL_THREADS, smem, st>>>(X, *os, *nl, U);
+    if (int rc = check_launch("ptar_os_null (prepare)")) return rc;
+  }
+  if (stage == 0 || stage == 2) {
+    static SmemOptIn optin;
+    if (int rc = opt_in_smem(ptar::os_null_gemm_kernel, optin, ptar::NL_SMEM, "ptar_os_null (GEMM)")) return rc;
+    const dim3 grid(static_cast<unsigned>(nl->n_colp / ptar::NL_BN), static_cast<unsigned>((nreal + ptar::NL_BM - 1) / ptar::NL_BM));
+    ptar::os_null_gemm_kernel<<<grid, ptar::NL_THREADS, ptar::NL_SMEM, st>>>(U, nreal, *nl, snr);
+    if (int rc = check_launch("ptar_os_null (GEMM)")) return rc;
+  }
+  if (stage == 0 || stage == 3) {
+    ptar::os_null_count_kernel<<<static_cast<unsigned>(nreal), ptar::NL_THREADS, 0, st>>>(snr, nl->n_col, exceed, fap);
+    if (int rc = check_launch("ptar_os_null (count)")) return rc;
+  }
+  return 0;
+}
+
+int ptar_os_null(const double* X, int32_t nreal, const ptar_os_model* os, const ptar_os_null_model* nl, double* U,
+                 double* snr, int64_t* exceed, double* fap, void* stream) {
+  return ptar_os_null_stage(X, nreal, os, nl, U, snr, exceed, fap, 0, stream);
 }
 
 int ptar_run_job_tm(const ptar_job* job, const ptar_timing_model* tm, double* scratch, int64_t scratch_len, int64_t real0,
