@@ -31,6 +31,8 @@
  *   ptar_os_project /      no counterpart: the frequentist optimal statistic of the realizations, reduced on the
  *   ptar_os_pairs          device instead of gathering the rows
  *   ptar_os_null           no counterpart: phase-shift / sky-scramble null distribution and p-value per realization
+ *   ptar_fp_project /      no counterpart: the incoherent Fp-statistic of continuous waves per realization and search
+ *   ptar_fp_reduce         frequency, reduced on the device
  */
 #ifndef PTAR_H
 #define PTAR_H
@@ -44,9 +46,10 @@ extern "C" {
 #define PTAR_VERSION 200  /* major*100 + minor; 2.0: column-major grid, g_ldr / c_rows, int8 GWB entry points, pshift phases.
                              Later additions leave every 2.0 struct layout and entry point unchanged: the timing-model fit
                              (ptar_timing_model, ptar_timing_project[_stage], ptar_run_job[_to_host]_tm) and the optimal
-                             statistic (ptar_os_model, ptar_os_project[_stage], ptar_os_pairs) and its null distributions
-                             (ptar_os_null_model, ptar_os_null[_stage]) are new symbols only, so a caller detects them by
-                             looking the symbol up. */
+                             statistic (ptar_os_model, ptar_os_project[_stage], ptar_os_pairs), its null distributions
+                             (ptar_os_null_model, ptar_os_null[_stage]) and the Fp-statistic (ptar_fp_model,
+                             ptar_fp_project, ptar_fp_reduce, PTAR_FP_MAX_FREQ) are new symbols only, so a caller detects
+                             them by looking the symbol up. */
 
 /* Geometry limits of the fused generator kernel. */
 #define PTAR_TILE_TOAS   1024  /* TOAs per tile (256 threads x 4)            */
@@ -348,6 +351,36 @@ int ptar_os_null(const double* X, int32_t nreal, const ptar_os_model* os, const 
                  double* U, double* snr, int64_t* exceed, double* fap, void* stream);
 int ptar_os_null_stage(const double* X, int32_t nreal, const ptar_os_model* os, const ptar_os_null_model* null_model,
                        double* U, double* snr, int64_t* exceed, double* fap, int stage, void* stream);
+
+/* Incoherent Fp-statistic (csrc/ptar_fp.cuh).  The host derives, once per recipe, for every pulsar a and search
+ * frequency f the whitened basis C~_a(f) = P_a^{-1} F_f L_a(f)^{-T} (F_f = (sin, cos)(2 pi f t), P_a the noise
+ * covariance with the timing model marginalised, L_a(f) L_a(f)^T = F_f^T P_a^{-1} F_f).  Per realization r:
+ *   ptar_fp_project  amps[r][a][j] = sum_i Ct_a[i][j] rows[r][i] over the TOAs i of pulsar a, j = 2 f + c < 2 n_freq:
+ *                    one fp64 tensor-core GEMM launch, one CTA per (pulsar, 64 realizations, 64 columns) walking all of
+ *                    the pulsar's TOAs, no partial sums.  rows: ld % 4 == 0, 32-byte aligned; alignment slots ignored.
+ *   ptar_fp_reduce   Fp[r][f] = 1/2 sum_a (amps[r][a][2f]^2 + amps[r][a][2f+1]^2), the sum in pulsar order;
+ *                    Fp_max[r] = max_f Fp[r][f], Fp_argmax[r] = the first f attaining it.
+ * Every sum runs in an order fixed by the TOA index and the pulsar only: outputs are bit-identical whatever nreal,
+ * chunking, real0 or launch grid produced the rows. */
+#define PTAR_FP_MAX_FREQ 256   /* search frequencies (the reduce kernel: one thread per frequency) */
+typedef struct {
+  int32_t n_psr;
+  int32_t n_freq;             /* Nf: 1 .. PTAR_FP_MAX_FREQ                                                         */
+  int32_t n_cb;               /* column blocks of 64: ceil(2 Nf / 64)                                              */
+  int32_t reserved;
+  int64_t ld;                 /* TOA pitch of Ct (the packed axis)                                                 */
+  const double* Ct;           /* [n_cb][ld][64]: Ct[b][i][(n + 8 (i & 1)) & 63] = C~[i][64 b + n] of the TOA's pulsar;
+                                 zero in alignment slots and columns >= 2 Nf                                       */
+  const int32_t* psr_order;   /* [n_psr] pulsars in grid order (descending TOA count: the longest CTAs start first) */
+  const int64_t* seg_off;     /* [n_psr] packed index of the pulsar's first TOA (multiple of 4)                    */
+  const int32_t* seg_len;     /* [n_psr] TOAs of the pulsar                                                        */
+} ptar_fp_model;
+
+/* amps: [nreal][n_psr][2 n_freq]. */
+int ptar_fp_project(const double* rows, int64_t ld, int32_t nreal, const ptar_fp_model* fp, double* amps, void* stream);
+/* Fp: [nreal][n_freq]; Fp_max, Fp_argmax: [nreal]. */
+int ptar_fp_reduce(const double* amps, int32_t nreal, const ptar_fp_model* fp, double* Fp, double* Fp_max,
+                   int64_t* Fp_argmax, void* stream);
 
 /* End-to-end job: GWB mix + synth + generate for realizations [real0, real0+nreal), then
  * (ptar_run_job_to_host) copy the residuals to pinned host memory, chunk by chunk, with the

@@ -12,6 +12,7 @@
 #include "ptar_generate.cuh"
 #include "ptar_gwb.cuh"
 #include "ptar_gwb_i8.cuh"
+#include "ptar_fp.cuh"
 #include "ptar_os.cuh"
 #include "ptar_os_null.cuh"
 #include "ptar_rng.cuh"
@@ -733,6 +734,38 @@ int ptar_os_null_stage(const double* X, int32_t nreal, const ptar_os_model* os, 
 int ptar_os_null(const double* X, int32_t nreal, const ptar_os_model* os, const ptar_os_null_model* nl, double* U,
                  double* snr, int64_t* exceed, double* fap, void* stream) {
   return ptar_os_null_stage(X, nreal, os, nl, U, snr, exceed, fap, 0, stream);
+}
+
+static int fp_model_check(const ptar_fp_model* fp, const char* what) {
+  if (!fp->Ct || !fp->psr_order || !fp->seg_off || !fp->seg_len || fp->n_psr <= 0 || fp->ld <= 0)
+    return fail(-2, "%s: model arrays missing", what);
+  if (fp->n_freq <= 0 || fp->n_freq > PTAR_FP_MAX_FREQ || fp->n_cb != (2 * fp->n_freq + ptar::FP_BN - 1) / ptar::FP_BN)
+    return fail(-2, "%s: need 1 <= n_freq <= 256 and n_cb = ceil(2 n_freq / 64)", what);
+  return 0;
+}
+
+int ptar_fp_project(const double* rows, int64_t ld, int32_t nreal, const ptar_fp_model* fp, double* amps, void* stream) {
+  if (!rows || !fp || !amps || nreal <= 0 || ld <= 0) return fail(-1, "ptar_fp_project: bad argument%s");
+  if (int rc = fp_model_check(fp, "ptar_fp_project")) return rc;
+  if ((ld & 3) || (reinterpret_cast<uintptr_t>(rows) & 31) || (reinterpret_cast<uintptr_t>(fp->Ct) & 15))
+    return fail(-2, "ptar_fp_project: rows must be 32-byte aligned with ld %% 4 == 0, Ct 16-byte aligned%s");
+  const int64_t blocks = int64_t(fp->n_psr) * ((nreal + ptar::OS_RB - 1) / ptar::OS_RB) * fp->n_cb;
+  if (blocks > 0x7fffffff) return fail(-3, "ptar_fp_project: grid too large%s");
+  static SmemOptIn optin;
+  if (int rc = opt_in_smem(ptar::fp_project_kernel, optin, ptar::FP_SMEM, "ptar_fp_project")) return rc;
+  ptar::fp_project_kernel<<<static_cast<unsigned>(blocks), ptar::FP_THREADS, ptar::FP_SMEM, static_cast<cudaStream_t>(stream)>>>(
+      rows, ld, nreal, *fp, amps);
+  return check_launch("ptar_fp_project");
+}
+
+int ptar_fp_reduce(const double* amps, int32_t nreal, const ptar_fp_model* fp, double* Fp, double* Fp_max,
+                   int64_t* Fp_argmax, void* stream) {
+  if (!amps || !fp || !Fp || !Fp_max || !Fp_argmax || nreal <= 0) return fail(-1, "ptar_fp_reduce: bad argument%s");
+  if (int rc = fp_model_check(fp, "ptar_fp_reduce")) return rc;
+  if (reinterpret_cast<uintptr_t>(amps) & 15) return fail(-2, "ptar_fp_reduce: amps must be 16-byte aligned%s");
+  ptar::fp_reduce_kernel<<<static_cast<unsigned>(nreal), ptar::FP_REDUCE_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(
+      amps, nreal, *fp, Fp, Fp_max, Fp_argmax);
+  return check_launch("ptar_fp_reduce");
 }
 
 int ptar_run_job_tm(const ptar_job* job, const ptar_timing_model* tm, double* scratch, int64_t scratch_len, int64_t real0,
