@@ -48,7 +48,7 @@ extern "C" {
                              (ptar_timing_model, ptar_timing_project[_stage], ptar_run_job[_to_host]_tm) and the optimal
                              statistic (ptar_os_model, ptar_os_project[_stage], ptar_os_pairs), its null distributions
                              (ptar_os_null_model, ptar_os_null[_stage]) and the Fp-statistic (ptar_fp_model,
-                             ptar_fp_project, ptar_fp_reduce, PTAR_FP_MAX_FREQ) are new symbols only, so a caller detects
+                             ptar_fp_project, ptar_fp_reduce[_fap], PTAR_FP_MAX_FREQ) are new symbols only, so a caller detects
                              them by looking the symbol up. */
 
 /* Geometry limits of the fused generator kernel. */
@@ -381,6 +381,11 @@ int ptar_fp_project(const double* rows, int64_t ld, int32_t nreal, const ptar_fp
 /* Fp: [nreal][n_freq]; Fp_max, Fp_argmax: [nreal]. */
 int ptar_fp_reduce(const double* amps, int32_t nreal, const ptar_fp_model* fp, double* Fp, double* Fp_max,
                    int64_t* Fp_argmax, void* stream);
+/* ptar_fp_reduce and, when fap is not NULL, fap[r][f] = Q(n_psr, Fp[r][f]) = Gamma(n_psr, Fp) / Gamma(n_psr), the
+ * single-frequency false-alarm probability ([nreal][n_freq]).  Evaluated as the finite sum e^{-x} sum_{k < n_psr} x^k / k!
+ * from its largest term: relative error ~ (Fp + n_psr) 2^-53, deterministic per element. */
+int ptar_fp_reduce_fap(const double* amps, int32_t nreal, const ptar_fp_model* fp, double* Fp, double* Fp_max,
+                       int64_t* Fp_argmax, double* fap, void* stream);
 
 /* End-to-end job: GWB mix + synth + generate for realizations [real0, real0+nreal), then
  * (ptar_run_job_to_host) copy the residuals to pinned host memory, chunk by chunk, with the

@@ -26,7 +26,8 @@ EXPORTS = ("ptar_version", "ptar_last_error", "ptar_cholesky_lower", "ptar_fouri
            "ptar_gwb_mix", "ptar_gwb_synth", "ptar_gwb_mix_i8", "ptar_gwb_slice_i8", "ptar_gwb_synth_i8", "ptar_debug_i8_timestamps", "ptar_generate", "ptar_generate_stage", "ptar_philox_normals", "ptar_peer_export", "ptar_peer_open", "ptar_peer_close", "ptar_peer_copy", "ptar_run_job",
            "ptar_run_job_to_host", "ptar_timing_project", "ptar_timing_project_stage",
            "ptar_run_job_tm", "ptar_run_job_to_host_tm", "ptar_os_project", "ptar_os_project_stage", "ptar_os_pairs",
-           "ptar_os_null", "ptar_os_null_stage", "ptar_fp_project", "ptar_fp_reduce")
+           "ptar_os_null", "ptar_os_null_stage", "ptar_fp_project", "ptar_fp_reduce",
+           "ptar_fp_reduce_fap")
 OS_MAX_NC, OS_MAX_ORF, OS_MAX_PSR = 32, 4, 256     # optimal statistic: GW-basis columns, templates, pulsars (ptar.h)
 OS_MAX_NULL = 65536                                # null columns of ptar_os_null (PTAR_OS_MAX_NULL)
 OS_NULL_PHASE_SHIFT, OS_NULL_SKY_SCRAMBLE = 1, 2
@@ -141,6 +142,7 @@ def lib():
     L.ptar_os_null_stage.argtypes = [vp, C.c_int32, vp, vp, vp, vp, vp, vp, i32, vp]
     L.ptar_fp_project.argtypes = [vp, i64, C.c_int32, vp, vp, vp]                        # fp: address of an FpModel
     L.ptar_fp_reduce.argtypes = [vp, C.c_int32, vp, vp, vp, vp, vp]
+    L.ptar_fp_reduce_fap.argtypes = [vp, C.c_int32, vp, vp, vp, vp, vp, vp]
     for name in EXPORTS:
         if name not in ("ptar_version", "ptar_last_error"):
             getattr(L, name).restype = C.c_int

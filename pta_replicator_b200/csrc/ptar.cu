@@ -758,14 +758,19 @@ int ptar_fp_project(const double* rows, int64_t ld, int32_t nreal, const ptar_fp
   return check_launch("ptar_fp_project");
 }
 
-int ptar_fp_reduce(const double* amps, int32_t nreal, const ptar_fp_model* fp, double* Fp, double* Fp_max,
-                   int64_t* Fp_argmax, void* stream) {
+int ptar_fp_reduce_fap(const double* amps, int32_t nreal, const ptar_fp_model* fp, double* Fp, double* Fp_max,
+                       int64_t* Fp_argmax, double* fap, void* stream) {
   if (!amps || !fp || !Fp || !Fp_max || !Fp_argmax || nreal <= 0) return fail(-1, "ptar_fp_reduce: bad argument%s");
   if (int rc = fp_model_check(fp, "ptar_fp_reduce")) return rc;
   if (reinterpret_cast<uintptr_t>(amps) & 15) return fail(-2, "ptar_fp_reduce: amps must be 16-byte aligned%s");
   ptar::fp_reduce_kernel<<<static_cast<unsigned>(nreal), ptar::FP_REDUCE_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(
-      amps, nreal, *fp, Fp, Fp_max, Fp_argmax);
+      amps, nreal, *fp, Fp, Fp_max, Fp_argmax, fap);
   return check_launch("ptar_fp_reduce");
+}
+
+int ptar_fp_reduce(const double* amps, int32_t nreal, const ptar_fp_model* fp, double* Fp, double* Fp_max,
+                   int64_t* Fp_argmax, void* stream) {
+  return ptar_fp_reduce_fap(amps, nreal, fp, Fp, Fp_max, Fp_argmax, nullptr, stream);
 }
 
 int ptar_run_job_tm(const ptar_job* job, const ptar_timing_model* tm, double* scratch, int64_t scratch_len, int64_t real0,

@@ -141,11 +141,52 @@ __global__ void __launch_bounds__(FP_THREADS, 1) fp_project_kernel(const double*
   }
 }
 
-// One CTA per realization, thread f = frequency: Fp in pulsar order, then (max, first argmax) by a fixed tree.
+// Q(P, x) = Gamma(P, x) / Gamma(P) for an integer shape P >= 1: the single-frequency false-alarm probability of Fp
+// (Fp ~ Gamma(P, 1) under the null).  For integer P, Q(P, x) = sum_{k < P} t_k with t_k = e^{-x} x^k / k!, every term
+// positive.  The largest term t_m, m = min(P - 1, floor(x)), is evaluated in log space; the others follow from it by
+// the ratios k / x (down) and x / (k + 1) (up), all <= 1, so nothing overflows and nothing cancels:
+//   ln t_m = m ln(x / m) + (m - x) - 1/2 ln(2 pi m) - delta(m),   delta(m) = ln m! - (m + 1/2) ln m + m - 1/2 ln(2 pi)
+// with ln(x / m) = log1p((x - m) / m) (x - m exact for x < 2m) and delta by its Stirling series for m >= 16 (truncation
+// < 1e-16), ln m! of the exact m! below.  Relative error ~ (x + P) u, the conditioning of Q itself; no branch of a
+// general-shape algorithm (the DLMF 8.12 asymptotic series of Cephes igammac loses ~1e-9 where Fp ~ P).  A fixed loop of
+// P - 1 steps per (realization, frequency): the value depends on x and P only.
+__device__ __forceinline__ double fp_q_int(int P, double x) {
+  if (!(x > 0.0)) return x == 0.0 ? 1.0 : x;   // Q(P, 0) = 1; NaN stays NaN (Fp >= 0 otherwise)
+  if (x == INFINITY) return 0.0;
+  const int m = x < double(P - 1) ? static_cast<int>(floor(x)) : P - 1;
+  const double dm = double(m);
+  double L;
+  if (m == 0) {
+    L = -x;
+  } else if (m < 16) {
+    double f = 1.0;
+    for (int k = 2; k <= m; ++k) f *= double(k);   // exact: 15! < 2^53
+    L = fma(dm, log(x), -x) - log(f);
+  } else {
+    const double i1 = 1.0 / dm, i2 = i1 * i1;
+    const double delta = i1 * (1.0 / 12 - i2 * (1.0 / 360 - i2 * (1.0 / 1260 - i2 * (1.0 / 1680 - i2 * (1.0 / 1188)))));
+    L = dm * log1p((x - dm) / dm) + (dm - x) - (0.9189385332046727418 + 0.5 * log(dm)) - delta;
+  }
+  double s = 1.0, r = 1.0;
+  for (int k = m; k > 0; --k) {
+    r *= double(k) / x;
+    s += r;
+  }
+  r = 1.0;
+  for (int k = m + 1; k < P; ++k) {
+    r *= x / double(k);
+    s += r;
+  }
+  return exp(L) * s;
+}
+
+// One CTA per realization, thread f = frequency: Fp in pulsar order, then (max, first argmax) by a fixed tree; with
+// `fap` also the false-alarm probability Q(n_psr, Fp) per frequency.
 __global__ void __launch_bounds__(FP_REDUCE_THREADS) fp_reduce_kernel(const double* __restrict__ amps, int nreal,
                                                                       ptar_fp_model fp, double* __restrict__ Fp,
                                                                       double* __restrict__ Fp_max,
-                                                                      int64_t* __restrict__ Fp_argmax) {
+                                                                      int64_t* __restrict__ Fp_argmax,
+                                                                      double* __restrict__ fap) {
   __shared__ double sv[FP_REDUCE_THREADS];
   __shared__ int si[FP_REDUCE_THREADS];
   const int64_t r = blockIdx.x;
@@ -161,6 +202,7 @@ __global__ void __launch_bounds__(FP_REDUCE_THREADS) fp_reduce_kernel(const doub
     }
     v = __dmul_rn(0.5, s);
     Fp[r * nf + f] = v;
+    if (fap) fap[r * nf + f] = fp_q_int(fp.n_psr, v);
   }
   sv[f] = v;
   si[f] = f;
