@@ -106,7 +106,7 @@ def main():
         line["os_null"] = {"method": args.null, "n": args.n_null, "kd": kd, "kernel": "os_null_gemm_kernel (DMMA)",
                            "gemm_ms_per_step": kms["os_null_gemm"], "gemm_flop": 2.0 * R * ncol * kd,
                            "gemm_TFLOPs": tflops, "frac_of_67_TFLOPs": tflops / 67.0,
-                           "V_bytes": int(nl["dev"]["V"].numel()) * 8, "U_bytes_per_chunk": int(b._os_null_U.numel()) * 8,
+                           "V_bytes": int(nl["dev"]["V"].numel()) * 8, "U_bytes_per_chunk": int(b._scratch_bufs["os_null_U"].numel()) * 8,
                            "null_statics_s": nl["setup_s"]}
     print(json.dumps(line), flush=True)
 

@@ -17,6 +17,7 @@ TILE_TOAS = 1024
 TILE_EPOCHS = 64
 TOA_ALIGN = 4
 I8_SLICES, I8_BM, I8_BN, I8_BK = 6, 128, 32, 32   # int8 wgmma GWB synthesis tile (csrc/ptar_gwb_i8.cuh)
+MIX_I8_MAX_PSR = 72                                # pulsars of ptar_gwb_mix_i8, the fused int8 mix (8 * MX_MAXNT, ptar_gwb.cuh)
 
 F_WHITE, F_ECORR, F_RED, F_GWB, F_DET, F_WHITE1 = 1, 2, 4, 8, 16, 32
 TM_KMAX = 32                                       # timing-model columns per pulsar (PTAR_TM_KMAX)

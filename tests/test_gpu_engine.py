@@ -261,6 +261,23 @@ def test_two_kernel_schedule_with_32_realization_blocks_and_scratch_checks():
     b.split_epoch = False
 
 
+def test_cached_two_kernel_job_owns_its_epoch_scratch():
+    """generate -> generate_to_host -> generate in the two-kernel schedule: the job generate caches owns its Cbuf (the
+    epoch kernel's scratch is in that job's keep list), so the job generate_to_host builds in between cannot release it,
+    and both generate calls give the fused schedule's bits."""
+    import torch
+    _, spec = load_flags_case()
+    b = _batch(_psrs(spec), spec)
+    fused = b.generate(40, seed=3, real0=8)
+    b.split_epoch = True
+    first = b.generate(40, seed=3, real0=8)
+    host = b.generate_to_host(40, seed=3, real0=8, chunk=16)
+    second = b.generate(40, seed=3, real0=8)
+    assert torch.equal(first, fused) and torch.equal(second, fused) and torch.equal(host, fused.cpu())
+    job, keep, _ = b._job_cache
+    assert job.gen.Cbuf and job.gen.Cbuf in [t.data_ptr() for t in keep]
+
+
 def test_parity_mode_requires_draws_for_every_enabled_term():
     """inject= with a term missing must raise instead of silently drawing that term from Philox (ADVICE round 1)."""
     import torch
