@@ -387,6 +387,39 @@ int ptar_fp_reduce(const double* amps, int32_t nreal, const ptar_fp_model* fp, d
 int ptar_fp_reduce_fap(const double* amps, int32_t nreal, const ptar_fp_model* fp, double* Fp, double* Fp_max,
                        int64_t* Fp_argmax, double* fap, void* stream);
 
+/* Coherent Fe-statistic over a sky grid (csrc/ptar_fe.cuh), from the amplitudes X^ of ptar_fp_project.  The host
+ * derives, once per recipe, L_a(f) (M_a(f) = L L^T of the Fp plan), the Earth-term antenna patterns e_a(s) = (F+, Fx)
+ * of every pulsar a at every sky point s and, per (f, s), the inverse Cholesky factor of
+ * M4(f, s) = sum_a e_a e_a^T (x) M_a(f) (4 x 4, index 2 pol + c, c = 0 sin, 1 cos).  Per realization r:
+ *   ptar_fe_sky      N_a(f) = L_a(f) X^[r][a][f] (formed while the operand is staged), then the fp64 tensor-core GEMM
+ *                    N4[(f, r, c)][(s, pol)] = sum_a N_a(f)[c] e_a(s)[pol] (the sum in pulsar order) with the epilogue
+ *                    Fe[r][f][s] = 1/2 |L4^-1 N4|^2 in registers, and fmax[r][f] = max_s Fe, fargmax[r][f] = the first
+ *                    s attaining it.  maps != NULL also writes Fe [nreal][n_freq][n_sky]; otherwise no map is written.
+ *   ptar_fe_combine  fe_max[r] = max_f fmax[r][f]; argmax_f[r] = the first f attaining it, argmax_sky[r] = its fargmax.
+ * Outputs are bit-identical whatever nreal, chunking or real0 produced the amplitudes. */
+#define PTAR_FE_MAX_PSR 128     /* pulsars: the staged N tile and two antenna stages, 199 KB of shared memory at 128 */
+#define PTAR_FE_MAX_SKY 12288   /* sky points: 12 nside^2 at nside 32 */
+typedef struct {
+  int32_t n_psr;              /* 1 .. PTAR_FE_MAX_PSR                                                              */
+  int32_t n_freq;             /* as the Fp model                                                                   */
+  int32_t n_sky;              /* S: 1 .. PTAR_FE_MAX_SKY                                                           */
+  int32_t n_sb;               /* sky blocks of 32: ceil(S / 32)                                                    */
+  int32_t kp;                 /* n_psr rounded up to a multiple of 16                                              */
+  int32_t reserved;
+  const double* Lf;           /* [n_freq][n_psr][3]: l11, l21, l22 of M_a(f)                                       */
+  const double* ant;          /* [n_sb][kp][64]: ant[b][a][(j + 8 (a & 1)) & 63] = e_a(32 b + j / 2)[j & 1]; zero
+                                 past n_psr and n_sky                                                              */
+  const double* linv;         /* [n_freq][32 n_sb][10]: L4^-1 packed by rows (00, 10, 11, 20, 21, 22, 30 .. 33);
+                                 zero past n_sky                                                                   */
+} ptar_fe_model;
+
+/* amps: [nreal][n_psr][2 n_freq] (ptar_fp_project); fmax: [nreal][n_freq]; fargmax: [nreal][n_freq] int64. */
+int ptar_fe_sky(const double* amps, int32_t nreal, const ptar_fe_model* fe, double* fmax, int64_t* fargmax, double* maps,
+                void* stream);
+/* fe_max, argmax_f, argmax_sky: [nreal]. */
+int ptar_fe_combine(const double* fmax, const int64_t* fargmax, int32_t nreal, const ptar_fe_model* fe, double* fe_max,
+                    int64_t* argmax_f, int64_t* argmax_sky, void* stream);
+
 /* End-to-end job: GWB mix + synth + generate for realizations [real0, real0+nreal), then
  * (ptar_run_job_to_host) copy the residuals to pinned host memory, chunk by chunk, with the
  * copy of chunk c overlapping the generation of chunk c+1 on a second stream. */

@@ -28,12 +28,14 @@ EXPORTS = ("ptar_version", "ptar_last_error", "ptar_cholesky_lower", "ptar_fouri
            "ptar_run_job_to_host", "ptar_timing_project", "ptar_timing_project_stage",
            "ptar_run_job_tm", "ptar_run_job_to_host_tm", "ptar_os_project", "ptar_os_project_stage", "ptar_os_pairs",
            "ptar_os_null", "ptar_os_null_stage", "ptar_fp_project", "ptar_fp_reduce",
-           "ptar_fp_reduce_fap")
+           "ptar_fp_reduce_fap", "ptar_fe_sky", "ptar_fe_combine")
 OS_MAX_NC, OS_MAX_ORF, OS_MAX_PSR = 32, 4, 256     # optimal statistic: GW-basis columns, templates, pulsars (ptar.h)
 OS_MAX_NULL = 65536                                # null columns of ptar_os_null (PTAR_OS_MAX_NULL)
 OS_NULL_PHASE_SHIFT, OS_NULL_SKY_SCRAMBLE = 1, 2
 OS_NULL_BK, OS_NULL_BN = 32, 64                    # kd / column padding of ptar_os_null_model (csrc/ptar_os_null.cuh)
 FP_MAX_FREQ = 256                                  # search frequencies of the Fp-statistic (PTAR_FP_MAX_FREQ)
+FE_MAX_PSR, FE_MAX_SKY = 128, 12288                # Fe-statistic: pulsars (shared-memory tile), sky points (ptar.h)
+FE_SB = 32                                         # sky points per stage of ptar_fe_sky (csrc/ptar_fe.cuh)
 
 
 class Tile(C.Structure):
@@ -92,6 +94,11 @@ class FpModel(C.Structure):
                 ("seg_len", C.c_void_p)]
 
 
+class FeModel(C.Structure):
+    _fields_ = [("n_psr", C.c_int32), ("n_freq", C.c_int32), ("n_sky", C.c_int32), ("n_sb", C.c_int32),
+                ("kp", C.c_int32), ("reserved", C.c_int32), ("Lf", C.c_void_p), ("ant", C.c_void_p), ("linv", C.c_void_p)]
+
+
 _lib = None
 
 
@@ -144,6 +151,8 @@ def lib():
     L.ptar_fp_project.argtypes = [vp, i64, C.c_int32, vp, vp, vp]                        # fp: address of an FpModel
     L.ptar_fp_reduce.argtypes = [vp, C.c_int32, vp, vp, vp, vp, vp]
     L.ptar_fp_reduce_fap.argtypes = [vp, C.c_int32, vp, vp, vp, vp, vp, vp]
+    L.ptar_fe_sky.argtypes = [vp, C.c_int32, vp, vp, vp, vp, vp]                         # fe: address of an FeModel
+    L.ptar_fe_combine.argtypes = [vp, vp, C.c_int32, vp, vp, vp, vp, vp]
     for name in EXPORTS:
         if name not in ("ptar_version", "ptar_last_error"):
             getattr(L, name).restype = C.c_int

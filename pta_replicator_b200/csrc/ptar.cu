@@ -12,6 +12,7 @@
 #include "ptar_generate.cuh"
 #include "ptar_gwb.cuh"
 #include "ptar_gwb_i8.cuh"
+#include "ptar_fe.cuh"
 #include "ptar_fp.cuh"
 #include "ptar_os.cuh"
 #include "ptar_os_null.cuh"
@@ -771,6 +772,42 @@ int ptar_fp_reduce_fap(const double* amps, int32_t nreal, const ptar_fp_model* f
 int ptar_fp_reduce(const double* amps, int32_t nreal, const ptar_fp_model* fp, double* Fp, double* Fp_max,
                    int64_t* Fp_argmax, void* stream) {
   return ptar_fp_reduce_fap(amps, nreal, fp, Fp, Fp_max, Fp_argmax, nullptr, stream);
+}
+
+static int fe_model_check(const ptar_fe_model* fe, const char* what) {
+  if (!fe->Lf || !fe->ant || !fe->linv) return fail(-2, "%s: model arrays missing", what);
+  if (fe->n_psr < 1 || fe->n_psr > PTAR_FE_MAX_PSR || fe->kp != ((fe->n_psr + 15) & ~15))
+    return fail(-2, "%s: need 1 <= n_psr <= 128 and kp = n_psr rounded up to a multiple of 16", what);
+  if (fe->n_freq < 1 || fe->n_freq > PTAR_FP_MAX_FREQ) return fail(-2, "%s: need 1 <= n_freq <= 256", what);
+  if (fe->n_sky < 1 || fe->n_sky > PTAR_FE_MAX_SKY || fe->n_sb != (fe->n_sky + ptar::FE_SB - 1) / ptar::FE_SB)
+    return fail(-2, "%s: need 1 <= n_sky <= 12288 and n_sb = ceil(n_sky / 32)", what);
+  if ((reinterpret_cast<uintptr_t>(fe->ant) & 15) || (reinterpret_cast<uintptr_t>(fe->linv) & 15))
+    return fail(-2, "%s: ant and linv must be 16-byte aligned", what);
+  return 0;
+}
+
+int ptar_fe_sky(const double* amps, int32_t nreal, const ptar_fe_model* fe, double* fmax, int64_t* fargmax, double* maps,
+                void* stream) {
+  if (!amps || !fe || !fmax || !fargmax || nreal <= 0) return fail(-1, "ptar_fe_sky: bad argument%s");
+  if (int rc = fe_model_check(fe, "ptar_fe_sky")) return rc;
+  if (reinterpret_cast<uintptr_t>(amps) & 15) return fail(-2, "ptar_fe_sky: amps must be 16-byte aligned%s");
+  static SmemOptIn optin;
+  if (int rc = opt_in_smem(ptar::fe_sky_kernel, optin, ptar::fe_smem_bytes(PTAR_FE_MAX_PSR), "ptar_fe_sky")) return rc;
+  const dim3 grid(static_cast<unsigned>((nreal + ptar::FE_RB - 1) / ptar::FE_RB), static_cast<unsigned>(fe->n_freq));
+  ptar::fe_sky_kernel<<<grid, ptar::FE_THREADS, ptar::fe_smem_bytes(fe->kp), static_cast<cudaStream_t>(stream)>>>(
+      amps, nreal, *fe, fmax, fargmax, maps);
+  return check_launch("ptar_fe_sky");
+}
+
+int ptar_fe_combine(const double* fmax, const int64_t* fargmax, int32_t nreal, const ptar_fe_model* fe, double* fe_max,
+                    int64_t* argmax_f, int64_t* argmax_sky, void* stream) {
+  if (!fmax || !fargmax || !fe || !fe_max || !argmax_f || !argmax_sky || nreal <= 0)
+    return fail(-1, "ptar_fe_combine: bad argument%s");
+  if (int rc = fe_model_check(fe, "ptar_fe_combine")) return rc;
+  const unsigned blocks = static_cast<unsigned>((nreal + ptar::FE_COMBINE_THREADS - 1) / ptar::FE_COMBINE_THREADS);
+  ptar::fe_combine_kernel<<<blocks, ptar::FE_COMBINE_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(
+      fmax, fargmax, nreal, fe->n_freq, fe_max, argmax_f, argmax_sky);
+  return check_launch("ptar_fe_combine");
 }
 
 int ptar_run_job_tm(const ptar_job* job, const ptar_timing_model* tm, double* scratch, int64_t scratch_len, int64_t real0,
