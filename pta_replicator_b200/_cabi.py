@@ -18,6 +18,29 @@ TILE_EPOCHS = 64
 TOA_ALIGN = 4
 I8_SLICES, I8_BM, I8_BN, I8_BK = 6, 128, 32, 32   # int8 wgmma GWB synthesis tile (csrc/ptar_gwb_i8.cuh)
 MIX_I8_MAX_PSR = 72                                # pulsars of ptar_gwb_mix_i8, the fused int8 mix (8 * MX_MAXNT, ptar_gwb.cuh)
+MIX_MAX_PSR = 112                                  # pulsars of ptar_gwb_mix: M and the draws of one item in 227 KB of shared memory
+SMEM_MAX = 227 * 1024                              # dynamic shared memory per block (sm_90)
+EPK_RB = 32                                        # realizations per CTA of the two-kernel schedule's epoch kernel
+
+
+def gen_smem_bytes(J, rc):
+    """Shared memory of the fused generator / its epoch stage at rc realizations (gen_smem_bytes, ptar_generate.cuh)."""
+    return 16 + 8 * max(J * TILE_EPOCHS + 3 * J * rc, TILE_EPOCHS * (3 * rc + 2))
+
+
+def epoch_smem_bytes(J):
+    """Shared memory of the standalone epoch kernel (epoch_smem_bytes, ptar_generate.cuh)."""
+    return 16 + 8 * (max(J * TILE_EPOCHS + 3 * J * EPK_RB, 3 * 24 * 64) + TILE_EPOCHS * EPK_RB * 2)
+
+
+def max_red_columns(rc=16, split_epoch=False):
+    """The largest (even) red-noise basis width J whose epoch stage fits shared memory in the given schedule: 258 fused at
+    rc = 16, 180 at rc = 32 (fused or two-kernel), 154 in the two-kernel schedule's epoch kernel (rc = 16)."""
+    need = epoch_smem_bytes if (split_epoch and rc != 32) else (lambda J: gen_smem_bytes(J, rc or 16))
+    J = 2
+    while need(J + 2) <= SMEM_MAX:
+        J += 2
+    return J
 
 F_WHITE, F_ECORR, F_RED, F_GWB, F_DET, F_WHITE1 = 1, 2, 4, 8, 16, 32
 TM_KMAX = 32                                       # timing-model columns per pulsar (PTAR_TM_KMAX)

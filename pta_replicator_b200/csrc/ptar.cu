@@ -309,9 +309,10 @@ template <bool INJECT, bool SLICE>
 int launch_mix(double* Zm, const double* M, const double* zin, int n_psr, int J, int64_t nreal, uint64_t seed, int64_t real0,
                int8_t* ZS, const double* zinv, int Jpad, int64_t rcap, cudaStream_t st, const char* what) {
   const int KP = (n_psr + 3) & ~3, NP = (n_psr + 7) & ~7;
-  // draws [KP][132] + M [NP][KP + 4] doubles: 113 KB at 67 pulsars (2 CTAs per SM), the 227 KB limit is reached at 115 pulsars
+  // draws [KP][132] + M [NP][KP + 4] doubles: 113 KB at 67 pulsars (2 CTAs per SM), 217 KB at 112 pulsars; 113 pulsars pad
+  // to KP = 116, NP = 120 (232 KB) and no longer fit the 227 KB limit (_cabi.MIX_MAX_PSR)
   const size_t smem = sizeof(double) * (size_t(KP) * ptar::MX_ZS + size_t(NP) * (KP + 4));
-  if (smem > 227 * 1024) return fail(-3, "ptar_gwb_mix: more than 115 pulsars do not fit the shared-memory tile%s");
+  if (smem > 227 * 1024) return fail(-3, "ptar_gwb_mix: more than 112 pulsars do not fit the shared-memory tile%s");
   static SmemOptIn optin;   // per instantiation
   if (int rc = opt_in_smem(ptar::gwb_mix_dmma_kernel<INJECT, SLICE>, optin, 227 * 1024, what)) return rc;
   // persistent: as many CTAs as are resident at once, each stages M once and loops over (column block, group) items
