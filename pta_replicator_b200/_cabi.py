@@ -16,7 +16,7 @@ LIB_PATH = os.environ.get("PTAR_B200_LIB") or os.path.join(_HERE, "csrc", "libpt
 TILE_TOAS = 1024
 TILE_EPOCHS = 64
 TOA_ALIGN = 4
-I8_SLICES, I8_BM, I8_BN, I8_BK = 6, 128, 32, 32   # int8 wgmma GWB synthesis tile (csrc/ptar_gwb_i8.cuh)
+I8_SLICES, I8_BM, I8_BN, I8_BK = 6, 128, 48, 32   # int8 wgmma GWB synthesis: ZS r-block, knots per tile, k-chunk (csrc/ptar_gwb_i8.cuh)
 MIX_I8_MAX_PSR = 72                                # pulsars of ptar_gwb_mix_i8, the fused int8 mix (8 * MX_MAXNT, ptar_gwb.cuh)
 MIX_MAX_PSR = 112                                  # pulsars of ptar_gwb_mix: M and the draws of one item in 227 KB of shared memory
 SMEM_MAX = 227 * 1024                              # dynamic shared memory per block (sm_90)

@@ -472,7 +472,7 @@ int ptar_gwb_synth_i8(double* G, int64_t g_ld, int64_t g_ldr, const int8_t* AS, 
   if (n_tiles > 65535) return fail(-3, "ptar_gwb_synth_i8: more than 65535 tiles%s");
   static SmemOptIn optin;
   if (int rc = opt_in_smem(ptar::gwb_synth_i8_kernel, optin, ptar::I8_SMEM, "ptar_gwb_synth_i8")) return rc;
-  const dim3 grid(static_cast<unsigned>((nreal + ptar::I8_BM - 1) / ptar::I8_BM), static_cast<unsigned>(n_tiles));
+  const dim3 grid(static_cast<unsigned>((nreal + ptar::I8_CM - 1) / ptar::I8_CM), static_cast<unsigned>(n_tiles));
   ptar::gwb_synth_i8_kernel<<<grid, ptar::I8_THREADS, ptar::I8_SMEM, static_cast<cudaStream_t>(stream)>>>(
       G, g_ld, g_ldr, AS, colscale, ZS, zscale, n_psr, J, Jpad, nreal, rcap, tile_list);
   return check_launch("ptar_gwb_synth_i8");
