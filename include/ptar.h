@@ -33,6 +33,8 @@
  *   ptar_os_null           no counterpart: phase-shift / sky-scramble null distribution and p-value per realization
  *   ptar_fp_project /      no counterpart: the incoherent Fp-statistic of continuous waves per realization and search
  *   ptar_fp_reduce         frequency, reduced on the device
+ *   ptar_curn_grid /       no counterpart (an MCMC over enterprise's CURN model per realization): the common-process
+ *   ptar_curn_reduce       likelihood on an (A, gamma) grid, its maximum, Bayes factor, marginals and upper limit
  */
 #ifndef PTAR_H
 #define PTAR_H
@@ -47,9 +49,10 @@ extern "C" {
                              Later additions leave every 2.0 struct layout and entry point unchanged: the timing-model fit
                              (ptar_timing_model, ptar_timing_project[_stage], ptar_run_job[_to_host]_tm) and the optimal
                              statistic (ptar_os_model, ptar_os_project[_stage], ptar_os_pairs), its null distributions
-                             (ptar_os_null_model, ptar_os_null[_stage]) and the Fp-statistic (ptar_fp_model,
-                             ptar_fp_project, ptar_fp_reduce[_fap], PTAR_FP_MAX_FREQ) are new symbols only, so a caller detects
-                             them by looking the symbol up. */
+                             (ptar_os_null_model, ptar_os_null[_stage]), the Fp-statistic (ptar_fp_model,
+                             ptar_fp_project, ptar_fp_reduce[_fap], PTAR_FP_MAX_FREQ) and the CURN likelihood
+                             (ptar_curn_model, ptar_curn_grid, ptar_curn_reduce, PTAR_CURN_MAX_NA / _NG) are new symbols
+                             only, so a caller detects them by looking the symbol up. */
 
 /* Geometry limits of the fused generator kernel. */
 #define PTAR_TILE_TOAS   1024  /* TOAs per tile (256 threads x 4)            */
@@ -419,6 +422,50 @@ int ptar_fe_sky(const double* amps, int32_t nreal, const ptar_fe_model* fe, doub
 /* fe_max, argmax_f, argmax_sky: [nreal]. */
 int ptar_fe_combine(const double* fmax, const int64_t* fargmax, int32_t nreal, const ptar_fe_model* fe, double* fe_max,
                     int64_t* argmax_f, int64_t* argmax_sky, void* stream);
+
+/* Common uncorrelated red process (CURN) likelihood on an (A, gamma) grid (csrc/ptar_curn.cuh), from the X of
+ * ptar_os_project run with a ptar_os_model that holds only the projection fields (tiles, tile0, n_tile, C, nc, ncp).
+ * The host derives, once per recipe, for every pulsar a and grid gamma the eigendecomposition
+ * phi~^{1/2} Z_a phi~^{1/2} = U diag(lambda) U^T (Z_a = F^T P_a^{-1} F, phi~ the power law at A = 1 and gamma),
+ * V_a(gamma) = U^T phi~^{1/2}, ldet[g][k] = sum_a sum_j log1p(A_k^2 lambda_j), and the trapezoid weights and prior of
+ * the grid.  Per realization r:
+ *   ptar_curn_grid    lnL[r][g][k] = 1/2 sum_a sum_j w_j y_j^2 - 1/2 ldet[g][k],  y = V_a(gamma_g) X[r][a],
+ *                     w_j = A_k^2 / (1 + A_k^2 lambda_j): two chained GEMMs on the fp64 tensor cores, the pulsar sum in
+ *                     index order.  X: [nreal][n_psr][ncp], 32-byte aligned.
+ *   ptar_curn_reduce  lnL_max[r], its first (g, k) (gamma-major) in ml_gamma[r], ml_amp[r];
+ *                     ln_bayes[r] = ln sum_{g,k} wg_g wx_k prior_k exp(lnL[r][g][k]);
+ *                     post_amp[r][k] = sum_g wg_g prior_k exp(lnL) / B;  post_gamma[r][g] = sum_k wx_k prior_k exp(lnL) / B;
+ *                     ul_amp[r] = the quantile ul of the trapezoid CDF of post_amp over log10_A, linear between nodes.
+ * Every sum runs in an order fixed by the pulsar, the grid index and the realization's own data: outputs are
+ * bit-identical whatever nreal, chunking or real0. */
+#define PTAR_CURN_MAX_NA 256    /* log10 A grid points (one reduce thread per point) */
+#define PTAR_CURN_MAX_NG 256    /* gamma grid points                                 */
+typedef struct {
+  int32_t n_psr;
+  int32_t nc;                 /* 2K <= PTAR_OS_MAX_NC                                                              */
+  int32_t ncp;                /* nc rounded up to a multiple of 8 (as the ptar_os_model of the projection)         */
+  int32_t n_gamma;            /* 1 .. PTAR_CURN_MAX_NG                                                             */
+  int32_t n_amp;              /* 2 .. PTAR_CURN_MAX_NA                                                             */
+  int32_t reserved;
+  const double* V;            /* [n_psr][n_gamma][ncp][ncp]: row j = eigenvector j of phi~^1/2 Z_a phi~^1/2 times
+                                 phi~^1/2; zero in rows and columns >= nc                                          */
+  const double* lam;          /* [n_psr][n_gamma][ncp]: eigenvalues (>= 0), zero past nc                           */
+  const double* a2;           /* [n_amp] A^2 = 10^(2 log10_A)                                                      */
+  const double* ldet;         /* [n_gamma][n_amp]                                                                  */
+  const double* log10_A;      /* [n_amp] strictly increasing                                                       */
+  const double* wg;           /* [n_gamma] trapezoid weights in gamma (1 for one point)                            */
+  const double* wx;           /* [n_amp] trapezoid weights in log10 A                                              */
+  const double* prior;        /* [n_amp] prior density, normalised: sum_g sum_k wg wx prior = 1                    */
+  double ul;                  /* upper-limit quantile in (0, 1)                                                    */
+} ptar_curn_model;
+
+/* lnL: [nreal][n_gamma][n_amp]. */
+int ptar_curn_grid(const double* X, int32_t nreal, const ptar_curn_model* cm, double* lnL, void* stream);
+/* lnL_max, ln_bayes, ul_amp: [nreal]; ml_gamma, ml_amp: [nreal] int64; post_amp: [nreal][n_amp];
+ * post_gamma: [nreal][n_gamma]. */
+int ptar_curn_reduce(const double* lnL, int32_t nreal, const ptar_curn_model* cm, double* lnL_max, int64_t* ml_gamma,
+                     int64_t* ml_amp, double* ln_bayes, double* post_amp, double* post_gamma, double* ul_amp,
+                     void* stream);
 
 /* End-to-end job: GWB mix + synth + generate for realizations [real0, real0+nreal), then
  * (ptar_run_job_to_host) copy the residuals to pinned host memory, chunk by chunk, with the

@@ -51,7 +51,7 @@ EXPORTS = ("ptar_version", "ptar_last_error", "ptar_cholesky_lower", "ptar_fouri
            "ptar_run_job_to_host", "ptar_timing_project", "ptar_timing_project_stage",
            "ptar_run_job_tm", "ptar_run_job_to_host_tm", "ptar_os_project", "ptar_os_project_stage", "ptar_os_pairs",
            "ptar_os_null", "ptar_os_null_stage", "ptar_fp_project", "ptar_fp_reduce",
-           "ptar_fp_reduce_fap", "ptar_fe_sky", "ptar_fe_combine")
+           "ptar_fp_reduce_fap", "ptar_fe_sky", "ptar_fe_combine", "ptar_curn_grid", "ptar_curn_reduce")
 OS_MAX_NC, OS_MAX_ORF, OS_MAX_PSR = 32, 4, 256     # optimal statistic: GW-basis columns, templates, pulsars (ptar.h)
 OS_MAX_NULL = 65536                                # null columns of ptar_os_null (PTAR_OS_MAX_NULL)
 OS_NULL_PHASE_SHIFT, OS_NULL_SKY_SCRAMBLE = 1, 2
@@ -59,6 +59,7 @@ OS_NULL_BK, OS_NULL_BN = 32, 64                    # kd / column padding of ptar
 FP_MAX_FREQ = 256                                  # search frequencies of the Fp-statistic (PTAR_FP_MAX_FREQ)
 FE_MAX_PSR, FE_MAX_SKY = 128, 12288                # Fe-statistic: pulsars (shared-memory tile), sky points (ptar.h)
 FE_SB = 32                                         # sky points per stage of ptar_fe_sky (csrc/ptar_fe.cuh)
+CURN_MAX_NA, CURN_MAX_NG = 256, 256                # CURN likelihood grid: log10 A and gamma points (ptar.h)
 
 
 class Tile(C.Structure):
@@ -122,6 +123,13 @@ class FeModel(C.Structure):
                 ("kp", C.c_int32), ("reserved", C.c_int32), ("Lf", C.c_void_p), ("ant", C.c_void_p), ("linv", C.c_void_p)]
 
 
+class CurnModel(C.Structure):
+    _fields_ = [("n_psr", C.c_int32), ("nc", C.c_int32), ("ncp", C.c_int32), ("n_gamma", C.c_int32),
+                ("n_amp", C.c_int32), ("reserved", C.c_int32), ("V", C.c_void_p), ("lam", C.c_void_p), ("a2", C.c_void_p),
+                ("ldet", C.c_void_p), ("log10_A", C.c_void_p), ("wg", C.c_void_p), ("wx", C.c_void_p),
+                ("prior", C.c_void_p), ("ul", C.c_double)]
+
+
 _lib = None
 
 
@@ -176,6 +184,8 @@ def lib():
     L.ptar_fp_reduce_fap.argtypes = [vp, C.c_int32, vp, vp, vp, vp, vp, vp]
     L.ptar_fe_sky.argtypes = [vp, C.c_int32, vp, vp, vp, vp, vp]                         # fe: address of an FeModel
     L.ptar_fe_combine.argtypes = [vp, vp, C.c_int32, vp, vp, vp, vp, vp]
+    L.ptar_curn_grid.argtypes = [vp, C.c_int32, vp, vp, vp]                           # cm: address of a CurnModel
+    L.ptar_curn_reduce.argtypes = [vp, C.c_int32, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     for name in EXPORTS:
         if name not in ("ptar_version", "ptar_last_error"):
             getattr(L, name).restype = C.c_int

@@ -9,6 +9,7 @@
 #include <algorithm>
 
 #include "../../include/ptar.h"
+#include "ptar_curn.cuh"
 #include "ptar_generate.cuh"
 #include "ptar_gwb.cuh"
 #include "ptar_gwb_i8.cuh"
@@ -809,6 +810,54 @@ int ptar_fe_combine(const double* fmax, const int64_t* fargmax, int32_t nreal, c
   ptar::fe_combine_kernel<<<blocks, ptar::FE_COMBINE_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(
       fmax, fargmax, nreal, fe->n_freq, fe_max, argmax_f, argmax_sky);
   return check_launch("ptar_fe_combine");
+}
+
+static int curn_model_check(const ptar_curn_model* cm, const char* what) {
+  if (!cm->V || !cm->lam || !cm->a2 || !cm->ldet || !cm->log10_A || !cm->wg || !cm->wx || !cm->prior || cm->n_psr <= 0)
+    return fail(-2, "%s: model arrays missing", what);
+  if (cm->nc <= 0 || cm->nc > PTAR_OS_MAX_NC || cm->ncp != ((cm->nc + 7) & ~7))
+    return fail(-2, "%s: need 0 < nc <= 32 and ncp = nc rounded up to a multiple of 8", what);
+  if (cm->n_amp < 2 || cm->n_amp > PTAR_CURN_MAX_NA || cm->n_gamma < 1 || cm->n_gamma > PTAR_CURN_MAX_NG)
+    return fail(-2, "%s: need 2 <= n_amp <= 256 and 1 <= n_gamma <= 256", what);
+  if (!(cm->ul > 0.0 && cm->ul < 1.0)) return fail(-2, "%s: need 0 < ul < 1", what);
+  return 0;
+}
+
+int ptar_curn_grid(const double* X, int32_t nreal, const ptar_curn_model* cm, double* lnL, void* stream) {
+  if (!X || !cm || !lnL || nreal <= 0) return fail(-1, "ptar_curn_grid: bad argument%s");
+  if (int rc = curn_model_check(cm, "ptar_curn_grid")) return rc;
+  if ((reinterpret_cast<uintptr_t>(X) & 31) || (reinterpret_cast<uintptr_t>(cm->V) & 15))
+    return fail(-2, "ptar_curn_grid: X must be 32-byte aligned, V 16-byte aligned%s");
+  const int64_t nrb = (int64_t(nreal) + ptar::CURN_RB - 1) / ptar::CURN_RB;
+  if (nrb > 65535) return fail(-3, "ptar_curn_grid: more than 65535 realization blocks%s");
+  const dim3 grid(static_cast<unsigned>((cm->n_amp + ptar::CURN_AB - 1) / ptar::CURN_AB), static_cast<unsigned>(nrb),
+                  static_cast<unsigned>(cm->n_gamma));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  static SmemOptIn optin[4];
+  switch (cm->ncp / 8) {
+#define PTAR_CURN_LAUNCH(NT)                                                                                           \
+  case NT:                                                                                                             \
+    if (int rc = opt_in_smem(ptar::curn_grid_kernel<NT>, optin[NT - 1], ptar::CURN_SMEM, "ptar_curn_grid")) return rc; \
+    ptar::curn_grid_kernel<NT><<<grid, ptar::CURN_THREADS, ptar::CURN_SMEM, st>>>(X, nreal, *cm, lnL);                 \
+    break;
+    PTAR_CURN_LAUNCH(1)
+    PTAR_CURN_LAUNCH(2)
+    PTAR_CURN_LAUNCH(3)
+    PTAR_CURN_LAUNCH(4)
+#undef PTAR_CURN_LAUNCH
+  }
+  return check_launch("ptar_curn_grid");
+}
+
+int ptar_curn_reduce(const double* lnL, int32_t nreal, const ptar_curn_model* cm, double* lnL_max, int64_t* ml_gamma,
+                     int64_t* ml_amp, double* ln_bayes, double* post_amp, double* post_gamma, double* ul_amp,
+                     void* stream) {
+  if (!lnL || !cm || !lnL_max || !ml_gamma || !ml_amp || !ln_bayes || !post_amp || !post_gamma || !ul_amp || nreal <= 0)
+    return fail(-1, "ptar_curn_reduce: bad argument%s");
+  if (int rc = curn_model_check(cm, "ptar_curn_reduce")) return rc;
+  ptar::curn_reduce_kernel<<<static_cast<unsigned>(nreal), ptar::CURN_RED_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(
+      lnL, nreal, *cm, lnL_max, ml_gamma, ml_amp, ln_bayes, post_amp, post_gamma, ul_amp);
+  return check_launch("ptar_curn_reduce");
 }
 
 int ptar_run_job_tm(const ptar_job* job, const ptar_timing_model* tm, double* scratch, int64_t scratch_len, int64_t real0,
