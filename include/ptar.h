@@ -35,6 +35,8 @@
  *   ptar_fp_reduce         frequency, reduced on the device
  *   ptar_curn_grid /       no counterpart (an MCMC over enterprise's CURN model per realization): the common-process
  *   ptar_curn_reduce       likelihood on an (A, gamma) grid, its maximum, Bayes factor, marginals and upper limit
+ *   ptar_hd_grid           no counterpart (an MCMC over enterprise's HD-correlated model per realization): the
+ *                          ORF-correlated common-process likelihood on the CURN grid, reduced by ptar_curn_reduce
  */
 #ifndef PTAR_H
 #define PTAR_H
@@ -50,9 +52,10 @@ extern "C" {
                              (ptar_timing_model, ptar_timing_project[_stage], ptar_run_job[_to_host]_tm) and the optimal
                              statistic (ptar_os_model, ptar_os_project[_stage], ptar_os_pairs), its null distributions
                              (ptar_os_null_model, ptar_os_null[_stage]), the Fp-statistic (ptar_fp_model,
-                             ptar_fp_project, ptar_fp_reduce[_fap], PTAR_FP_MAX_FREQ) and the CURN likelihood
-                             (ptar_curn_model, ptar_curn_grid, ptar_curn_reduce, PTAR_CURN_MAX_NA / _NG) are new symbols
-                             only, so a caller detects them by looking the symbol up. */
+                             ptar_fp_project, ptar_fp_reduce[_fap], PTAR_FP_MAX_FREQ), the CURN likelihood
+                             (ptar_curn_model, ptar_curn_grid, ptar_curn_reduce, PTAR_CURN_MAX_NA / _NG) and the HD
+                             likelihood (ptar_hd_model, ptar_hd_grid, PTAR_HD_MAX_N / _JB) are new symbols only, so a
+                             caller detects them by looking the symbol up. */
 
 /* Geometry limits of the fused generator kernel. */
 #define PTAR_TILE_TOAS   1024  /* TOAs per tile (256 threads x 4)            */
@@ -466,6 +469,36 @@ int ptar_curn_grid(const double* X, int32_t nreal, const ptar_curn_model* cm, do
 int ptar_curn_reduce(const double* lnL, int32_t nreal, const ptar_curn_model* cm, double* lnL_max, int64_t* ml_gamma,
                      int64_t* ml_amp, double* ln_bayes, double* post_amp, double* post_gamma, double* ul_amp,
                      void* stream);
+
+/* Hellings-Downs (ORF-correlated) common-process likelihood (csrc/ptar_hd.cuh) on the grid of a ptar_curn_model, from
+ * the same X.  With the ORF Gamma = B B^T (n_psr x n_psr, positive semi-definite) and G = B (x) phi~^{1/2}, the host
+ * derives once per recipe, for every grid gamma, the eigendecomposition G^T Z G = U diag(lambda) U^T of size
+ * n = n_psr nc (Z = blockdiag(Z_a)), V(gamma) = U^T G^T and ldet[g][k] = sum_j log1p(A_k^2 lambda_j).  Per realization r:
+ *   ptar_hd_grid  lnL[r][g][k] = 1/2 sum_j w_j y_j^2 - 1/2 ldet[g][k],  y = V(gamma_g) X[r] (X[r] stacked over the
+ *                 pulsars), w_j = A_k^2 / (1 + A_k^2 lambda_j): two chained GEMMs on the fp64 tensor cores, j and the
+ *                 stacked X axis in index order.  X: [nreal][n_psr][ncp], 32-byte aligned.
+ * The summaries of the map are ptar_curn_reduce's, with the ptar_curn_model of the grid.  Outputs are bit-identical
+ * whatever nreal, chunking or real0. */
+#define PTAR_HD_MAX_N 4096      /* n = n_psr nc eigen-rows                                    */
+#define PTAR_HD_JB    32        /* eigen-rows per block: np = n rounded up to a multiple of 32 */
+typedef struct {
+  int32_t n_psr;
+  int32_t nc;                 /* 2K <= PTAR_OS_MAX_NC                                                              */
+  int32_t ncp;                /* nc rounded up to a multiple of 8 (as the ptar_os_model of the projection)         */
+  int32_t n_gamma;            /* 1 .. PTAR_CURN_MAX_NG                                                             */
+  int32_t n_amp;              /* 2 .. PTAR_CURN_MAX_NA                                                             */
+  int32_t n;                  /* n_psr nc <= PTAR_HD_MAX_N                                                          */
+  int32_t np;                 /* n rounded up to a multiple of PTAR_HD_JB                                           */
+  int32_t reserved;
+  const double* V;            /* [n_gamma][np][n_psr][ncp]: row j = eigenvector j of G^T Z G times G^T; zero in rows
+                                 >= n and in the columns of each pulsar >= nc; 16-byte aligned                     */
+  const double* lam;          /* [n_gamma][np]: eigenvalues (>= 0), zero past n                                    */
+  const double* a2;           /* [n_amp] A^2 = 10^(2 log10_A)                                                      */
+  const double* ldet;         /* [n_gamma][n_amp]                                                                  */
+} ptar_hd_model;
+
+/* lnL: [nreal][n_gamma][n_amp]. */
+int ptar_hd_grid(const double* X, int32_t nreal, const ptar_hd_model* hm, double* lnL, void* stream);
 
 /* End-to-end job: GWB mix + synth + generate for realizations [real0, real0+nreal), then
  * (ptar_run_job_to_host) copy the residuals to pinned host memory, chunk by chunk, with the

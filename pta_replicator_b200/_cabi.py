@@ -51,7 +51,8 @@ EXPORTS = ("ptar_version", "ptar_last_error", "ptar_cholesky_lower", "ptar_fouri
            "ptar_run_job_to_host", "ptar_timing_project", "ptar_timing_project_stage",
            "ptar_run_job_tm", "ptar_run_job_to_host_tm", "ptar_os_project", "ptar_os_project_stage", "ptar_os_pairs",
            "ptar_os_null", "ptar_os_null_stage", "ptar_fp_project", "ptar_fp_reduce",
-           "ptar_fp_reduce_fap", "ptar_fe_sky", "ptar_fe_combine", "ptar_curn_grid", "ptar_curn_reduce")
+           "ptar_fp_reduce_fap", "ptar_fe_sky", "ptar_fe_combine", "ptar_curn_grid", "ptar_curn_reduce",
+           "ptar_hd_grid")
 OS_MAX_NC, OS_MAX_ORF, OS_MAX_PSR = 32, 4, 256     # optimal statistic: GW-basis columns, templates, pulsars (ptar.h)
 OS_MAX_NULL = 65536                                # null columns of ptar_os_null (PTAR_OS_MAX_NULL)
 OS_NULL_PHASE_SHIFT, OS_NULL_SKY_SCRAMBLE = 1, 2
@@ -60,6 +61,7 @@ FP_MAX_FREQ = 256                                  # search frequencies of the F
 FE_MAX_PSR, FE_MAX_SKY = 128, 12288                # Fe-statistic: pulsars (shared-memory tile), sky points (ptar.h)
 FE_SB = 32                                         # sky points per stage of ptar_fe_sky (csrc/ptar_fe.cuh)
 CURN_MAX_NA, CURN_MAX_NG = 256, 256                # CURN likelihood grid: log10 A and gamma points (ptar.h)
+HD_MAX_N, HD_JB = 4096, 32                         # HD likelihood: n_psr 2K eigen-rows, rows per block (ptar.h)
 
 
 class Tile(C.Structure):
@@ -130,6 +132,12 @@ class CurnModel(C.Structure):
                 ("prior", C.c_void_p), ("ul", C.c_double)]
 
 
+class HdModel(C.Structure):
+    _fields_ = [("n_psr", C.c_int32), ("nc", C.c_int32), ("ncp", C.c_int32), ("n_gamma", C.c_int32),
+                ("n_amp", C.c_int32), ("n", C.c_int32), ("np", C.c_int32), ("reserved", C.c_int32), ("V", C.c_void_p),
+                ("lam", C.c_void_p), ("a2", C.c_void_p), ("ldet", C.c_void_p)]
+
+
 _lib = None
 
 
@@ -186,6 +194,7 @@ def lib():
     L.ptar_fe_combine.argtypes = [vp, vp, C.c_int32, vp, vp, vp, vp, vp]
     L.ptar_curn_grid.argtypes = [vp, C.c_int32, vp, vp, vp]                           # cm: address of a CurnModel
     L.ptar_curn_reduce.argtypes = [vp, C.c_int32, vp, vp, vp, vp, vp, vp, vp, vp, vp]
+    L.ptar_hd_grid.argtypes = [vp, C.c_int32, vp, vp, vp]                             # hm: address of an HdModel
     for name in EXPORTS:
         if name not in ("ptar_version", "ptar_last_error"):
             getattr(L, name).restype = C.c_int

@@ -13,6 +13,7 @@
 #include "ptar_generate.cuh"
 #include "ptar_gwb.cuh"
 #include "ptar_gwb_i8.cuh"
+#include "ptar_hd.cuh"
 #include "ptar_fe.cuh"
 #include "ptar_fp.cuh"
 #include "ptar_os.cuh"
@@ -858,6 +859,37 @@ int ptar_curn_reduce(const double* lnL, int32_t nreal, const ptar_curn_model* cm
   ptar::curn_reduce_kernel<<<static_cast<unsigned>(nreal), ptar::CURN_RED_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(
       lnL, nreal, *cm, lnL_max, ml_gamma, ml_amp, ln_bayes, post_amp, post_gamma, ul_amp);
   return check_launch("ptar_curn_reduce");
+}
+
+int ptar_hd_grid(const double* X, int32_t nreal, const ptar_hd_model* hm, double* lnL, void* stream) {
+  if (!X || !hm || !lnL || nreal <= 0) return fail(-1, "ptar_hd_grid: bad argument%s");
+  if (!hm->V || !hm->lam || !hm->a2 || !hm->ldet || hm->n_psr <= 0) return fail(-2, "ptar_hd_grid: model arrays missing%s");
+  if (hm->nc <= 0 || hm->nc > PTAR_OS_MAX_NC || hm->ncp != ((hm->nc + 7) & ~7))
+    return fail(-2, "ptar_hd_grid: need 0 < nc <= 32 and ncp = nc rounded up to a multiple of 8%s");
+  if (int64_t(hm->n) != int64_t(hm->n_psr) * hm->nc || hm->n > PTAR_HD_MAX_N ||
+      hm->np != (hm->n + PTAR_HD_JB - 1) / PTAR_HD_JB * PTAR_HD_JB)
+    return fail(-2, "ptar_hd_grid: need n = n_psr nc <= 4096 and np = n rounded up to a multiple of 32%s");
+  if (hm->n_amp < 2 || hm->n_amp > PTAR_CURN_MAX_NA || hm->n_gamma < 1 || hm->n_gamma > PTAR_CURN_MAX_NG)
+    return fail(-2, "ptar_hd_grid: need 2 <= n_amp <= 256 and 1 <= n_gamma <= 256%s");
+  if ((reinterpret_cast<uintptr_t>(X) & 31) || (reinterpret_cast<uintptr_t>(hm->V) & 15))
+    return fail(-2, "ptar_hd_grid: X must be 32-byte aligned, V 16-byte aligned%s");
+  const int64_t nrb = (int64_t(nreal) + ptar::HD_RB - 1) / ptar::HD_RB;
+  const dim3 grid(static_cast<unsigned>(nrb), static_cast<unsigned>(hm->n_gamma));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  static SmemOptIn optin[3];
+  const int qn = hm->n_amp <= 64 ? 4 : hm->n_amp <= 128 ? 8 : 16;   // 16 QN amplitude columns per CTA
+  switch (qn) {
+#define PTAR_HD_LAUNCH(QN, I)                                                                                           \
+  case QN:                                                                                                              \
+    if (int rc = opt_in_smem(ptar::hd_grid_kernel<QN>, optin[I], ptar::hd_smem(QN), "ptar_hd_grid")) return rc;        \
+    ptar::hd_grid_kernel<QN><<<grid, ptar::HD_THREADS, ptar::hd_smem(QN), st>>>(X, nreal, *hm, lnL);                    \
+    break;
+    PTAR_HD_LAUNCH(4, 0)
+    PTAR_HD_LAUNCH(8, 1)
+    PTAR_HD_LAUNCH(16, 2)
+#undef PTAR_HD_LAUNCH
+  }
+  return check_launch("ptar_hd_grid");
 }
 
 int ptar_run_job_tm(const ptar_job* job, const ptar_timing_model* tm, double* scratch, int64_t scratch_len, int64_t real0,
