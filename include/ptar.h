@@ -31,6 +31,7 @@
  *   ptar_os_project /      no counterpart: the frequentist optimal statistic of the realizations, reduced on the
  *   ptar_os_pairs          device instead of gathering the rows
  *   ptar_os_null           no counterpart: phase-shift / sky-scramble null distribution and p-value per realization
+ *   ptar_os_aniso          no counterpart: spherical-harmonic fit, anisotropy chi^2 and radiometer sky map per realization
  *   ptar_fp_project /      no counterpart: the incoherent Fp-statistic of continuous waves per realization and search
  *   ptar_fp_reduce         frequency, reduced on the device
  *   ptar_curn_grid /       no counterpart (an MCMC over enterprise's CURN model per realization): the common-process
@@ -51,7 +52,8 @@ extern "C" {
                              Later additions leave every 2.0 struct layout and entry point unchanged: the timing-model fit
                              (ptar_timing_model, ptar_timing_project[_stage], ptar_run_job[_to_host]_tm) and the optimal
                              statistic (ptar_os_model, ptar_os_project[_stage], ptar_os_pairs), its null distributions
-                             (ptar_os_null_model, ptar_os_null[_stage]), the Fp-statistic (ptar_fp_model,
+                             (ptar_os_null_model, ptar_os_null[_stage]) and anisotropy (ptar_os_aniso_model,
+                             ptar_os_aniso[_stage], PTAR_OS_ANISO_MAX_LM / _SKY), the Fp-statistic (ptar_fp_model,
                              ptar_fp_project, ptar_fp_reduce[_fap], PTAR_FP_MAX_FREQ), the CURN likelihood
                              (ptar_curn_model, ptar_curn_grid, ptar_curn_reduce, PTAR_CURN_MAX_NA / _NG) and the HD
                              likelihood (ptar_hd_model, ptar_hd_grid, PTAR_HD_MAX_N / _JB) are new symbols only, so a
@@ -357,6 +359,41 @@ int ptar_os_null(const double* X, int32_t nreal, const ptar_os_model* os, const 
                  double* U, double* snr, int64_t* exceed, double* fap, void* stream);
 int ptar_os_null_stage(const double* X, int32_t nreal, const ptar_os_model* os, const ptar_os_null_model* null_model,
                        double* U, double* snr, int64_t* exceed, double* fap, int stage, void* stream);
+
+/* Anisotropy of the optimal statistic (csrc/ptar_os_aniso.cuh): spherical-harmonic fits and radiometer sky maps, from
+ * statics derived once on the host.  Per realization r, from the X of ptar_os_project, x = X phi~^{1/2} and the pair
+ * correlations d_q = x_a . x_b (q = (a, b) the pairs of os):
+ *   map[r][c] = (sum_q d_q V[q][c]) / dsqrt[c],  columns c = [c^_lm (n_lm) | z (n_z) | radiometer S/N (n_sky)]
+ *   clm[r][j] = map[r][j];  z[r][j] = map[r][n_lm + j];  chi2[r] = sum_j z[r][j]^2 (fixed tree);
+ *   snr_max[r] = max_k map[r][n_lm + n_z + k], argmax[r] = the first k attaining it (NaN ranks above every number);
+ *   radio_map[r][k] = map[r][n_lm + n_z + k] when radio_map is not NULL.
+ * Three launches: the prepare and GEMM of ptar_os_null (sky-scramble operands: kd = n_pairs) and the reduction.  Each
+ * output is summed in an order fixed by q only: outputs are bit-identical whatever nreal, chunking or real0.
+ * ptar_os_aniso_stage runs one launch (stage 1 = prepare, 2 = GEMM, 3 = reduce; 0 = all three). */
+#define PTAR_OS_ANISO_MAX_LM  64        /* spherical-harmonic coefficients: lmax <= 7 */
+#define PTAR_OS_ANISO_MAX_SKY 12288     /* radiometer pixels (HEALPix nside 32)       */
+typedef struct {
+  int32_t n_lm;             /* (lmax + 1)^2 coefficients, 0 without a spherical-harmonic basis                   */
+  int32_t n_z;              /* n_lm - 1 whitened anisotropy components (0 when n_lm <= 1)                         */
+  int32_t n_sky;            /* radiometer pixels, 0 without a radiometer; n_lm + n_sky >= 1                       */
+  int32_t n_col;            /* n_lm + n_z + n_sky                                                                  */
+  int32_t n_colp;           /* n_col rounded up to a multiple of 64                                                */
+  int32_t reserved;
+  int64_t kd;               /* n_pairs                                                                             */
+  int64_t kdp;              /* kd rounded up to a multiple of 32                                                   */
+  const double* V;          /* [n_colp][kdp]: V^T, row c = column c of V, zero past kd and in rows >= n_col        */
+  const double* dsqrt;      /* [n_col] column divisors (1 for c^ and z, sqrt(F_kk) for the radiometer)             */
+} ptar_os_aniso_model;
+
+/* U: scratch of nreal * kdp doubles; map: scratch [nreal][n_col]; clm [nreal][n_lm], z [nreal][n_z], chi2 [nreal]
+ * (may be NULL when n_lm = 0; z also when n_z = 0); snr_max [nreal], argmax [nreal] int64 (may be NULL when
+ * n_sky = 0); radio_map [nreal][n_sky] or NULL.  X and os as for ptar_os_pairs. */
+int ptar_os_aniso(const double* X, int32_t nreal, const ptar_os_model* os, const ptar_os_aniso_model* model, double* U,
+                  double* map, double* clm, double* z, double* chi2, double* snr_max, int64_t* argmax,
+                  double* radio_map, void* stream);
+int ptar_os_aniso_stage(const double* X, int32_t nreal, const ptar_os_model* os, const ptar_os_aniso_model* model,
+                        double* U, double* map, double* clm, double* z, double* chi2, double* snr_max, int64_t* argmax,
+                        double* radio_map, int stage, void* stream);
 
 /* Incoherent Fp-statistic (csrc/ptar_fp.cuh).  The host derives, once per recipe, for every pulsar a and search
  * frequency f the whitened basis C~_a(f) = P_a^{-1} F_f L_a(f)^{-T} (F_f = (sin, cos)(2 pi f t), P_a the noise

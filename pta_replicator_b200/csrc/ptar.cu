@@ -17,6 +17,7 @@
 #include "ptar_fe.cuh"
 #include "ptar_fp.cuh"
 #include "ptar_os.cuh"
+#include "ptar_os_aniso.cuh"
 #include "ptar_os_null.cuh"
 #include "ptar_rng.cuh"
 #include "ptar_timing.cuh"
@@ -738,6 +739,57 @@ int ptar_os_null_stage(const double* X, int32_t nreal, const ptar_os_model* os, 
 int ptar_os_null(const double* X, int32_t nreal, const ptar_os_model* os, const ptar_os_null_model* nl, double* U,
                  double* snr, int64_t* exceed, double* fap, void* stream) {
   return ptar_os_null_stage(X, nreal, os, nl, U, snr, exceed, fap, 0, stream);
+}
+
+int ptar_os_aniso_stage(const double* X, int32_t nreal, const ptar_os_model* os, const ptar_os_aniso_model* am, double* U,
+                        double* map, double* clm, double* z, double* chi2, double* snr_max, int64_t* argmax,
+                        double* radio_map, int stage, void* stream) {
+  if (!X || !os || !am || !U || !map || nreal <= 0 || stage < 0 || stage > 3) return fail(-1, "ptar_os_aniso: bad argument%s");
+  if (!os->sqrt_phi || !os->pairs || !am->V || !am->dsqrt) return fail(-2, "ptar_os_aniso: model arrays missing%s");
+  if (os->n_psr < 2 || os->n_psr > PTAR_OS_MAX_PSR || os->n_pairs != os->n_psr * (os->n_psr - 1) / 2)
+    return fail(-3, "ptar_os_aniso: need 2..256 pulsars and every pair%s");
+  if (os->nc <= 0 || os->nc > PTAR_OS_MAX_NC || os->ncp != ((os->nc + 7) & ~7))
+    return fail(-2, "ptar_os_aniso: need 0 < nc <= 32 and ncp = nc rounded up to a multiple of 8%s");
+  if (am->n_lm < 0 || am->n_lm > PTAR_OS_ANISO_MAX_LM || am->n_z != std::max(am->n_lm - 1, 0) || am->n_sky < 0 ||
+      am->n_sky > PTAR_OS_ANISO_MAX_SKY || am->n_lm + am->n_sky < 1)
+    return fail(-2, "ptar_os_aniso: need 0 <= n_lm <= 64, n_z = max(n_lm - 1, 0), 0 <= n_sky <= 12288 and a basis%s");
+  if (am->n_col != am->n_lm + am->n_z + am->n_sky || am->n_colp != ((am->n_col + ptar::NL_BN - 1) & ~(ptar::NL_BN - 1)))
+    return fail(-2, "ptar_os_aniso: need n_col = n_lm + n_z + n_sky and n_colp = n_col rounded up to a multiple of 64%s");
+  if (am->kd != os->n_pairs || am->kdp != ((am->kd + ptar::NL_BK - 1) & ~int64_t(ptar::NL_BK - 1)))
+    return fail(-2, "ptar_os_aniso: kd must be n_pairs and kdp kd rounded up to 32%s");
+  if ((am->n_lm > 0 && (!clm || !chi2 || (am->n_z > 0 && !z))) || (am->n_sky > 0 && (!snr_max || !argmax)))
+    return fail(-1, "ptar_os_aniso: an output of a registered basis is NULL%s");
+  // the sky-scramble operands of ptar_os_null: U[r][q] = x_a . x_b, V^T rows = the columns of the anisotropy map
+  const ptar_os_null_model nl{PTAR_OS_NULL_SKY_SCRAMBLE, am->n_col, am->n_colp, 0, am->kd, am->kdp, am->V, am->dsqrt};
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (stage == 0 || stage == 1) {
+    const size_t smem = sizeof(double) * size_t(os->n_psr) * os->ncp;
+    static SmemOptIn optin;
+    if (int rc = opt_in_smem(ptar::os_null_prepare_kernel, optin, sizeof(double) * size_t(PTAR_OS_MAX_PSR) * PTAR_OS_MAX_NC,
+                             "ptar_os_aniso (prepare)"))
+      return rc;
+    ptar::os_null_prepare_kernel<<<static_cast<unsigned>(nreal), ptar::NL_THREADS, smem, st>>>(X, *os, nl, U);
+    if (int rc = check_launch("ptar_os_aniso (prepare)")) return rc;
+  }
+  if (stage == 0 || stage == 2) {
+    static SmemOptIn optin;
+    if (int rc = opt_in_smem(ptar::os_null_gemm_kernel, optin, ptar::NL_SMEM, "ptar_os_aniso (GEMM)")) return rc;
+    const dim3 grid(static_cast<unsigned>(nl.n_colp / ptar::NL_BN), static_cast<unsigned>((nreal + ptar::NL_BM - 1) / ptar::NL_BM));
+    ptar::os_null_gemm_kernel<<<grid, ptar::NL_THREADS, ptar::NL_SMEM, st>>>(U, nreal, nl, map);
+    if (int rc = check_launch("ptar_os_aniso (GEMM)")) return rc;
+  }
+  if (stage == 0 || stage == 3) {
+    ptar::os_aniso_reduce_kernel<<<static_cast<unsigned>(nreal), ptar::AN_THREADS, 0, st>>>(map, *am, clm, z, chi2, snr_max,
+                                                                                          argmax, radio_map);
+    if (int rc = check_launch("ptar_os_aniso (reduce)")) return rc;
+  }
+  return 0;
+}
+
+int ptar_os_aniso(const double* X, int32_t nreal, const ptar_os_model* os, const ptar_os_aniso_model* am, double* U,
+                  double* map, double* clm, double* z, double* chi2, double* snr_max, int64_t* argmax, double* radio_map,
+                  void* stream) {
+  return ptar_os_aniso_stage(X, nreal, os, am, U, map, clm, z, chi2, snr_max, argmax, radio_map, 0, stream);
 }
 
 static int fp_model_check(const ptar_fp_model* fp, const char* what) {
