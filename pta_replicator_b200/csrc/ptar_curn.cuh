@@ -18,6 +18,7 @@
 // statics and the pulsar order only -- not on the realization block, nreal, chunking or real0.  No atomics.
 #pragma once
 #include <cuda_runtime.h>
+#include <math.h>
 #include <stdint.h>
 
 #include "../../include/ptar.h"
@@ -125,6 +126,9 @@ __global__ void __launch_bounds__(CURN_THREADS, 1) curn_grid_kernel(const double
 //   s_k = sum_g wg_g e_gk (in g order);  t_g = sum_k wx_k prior_k e_gk (in k order);  B' = tree_k wx_k prior_k s_k
 //   ln_bayes = m + ln B';  post_log10_A_k = prior_k s_k / B';  post_gamma_g = t_g / B'
 //   ul: the quantile `ul` of the trapezoid CDF of post_log10_A (normalised by its last node), linear between nodes.
+// Non-finite maps: the maximum ranks by fe_better (the first NaN above every number).  -inf among finite entries is a
+// zero likelihood; a NaN or +inf anywhere makes ln_bayes, both posteriors and ul NaN; an all -inf map gives m = -inf at
+// (0, 0), ln_bayes = -inf, posteriors and ul NaN.
 __global__ void __launch_bounds__(CURN_RED_THREADS) curn_reduce_kernel(const double* __restrict__ lnL, int nreal,
                                                                        ptar_curn_model cm, double* __restrict__ lmax,
                                                                        int64_t* __restrict__ ml_g, int64_t* __restrict__ ml_a,
@@ -137,23 +141,25 @@ __global__ void __launch_bounds__(CURN_RED_THREADS) curn_reduce_kernel(const dou
   const int64_t r = blockIdx.x;
   const double* m = lnL + r * n;
   double best = -INFINITY;
-  int bi = n;
+  int bi = INT32_MAX;   // ranks below every entry: a -inf entry still wins on its index
   for (int e = tid; e < n; e += CURN_RED_THREADS) {
     const double v = m[e];
-    if (v > best) best = v, bi = e;
+    if (fe_better(v, e, best, bi)) best = v, bi = e;
   }
   rv[tid] = best;
   ri[tid] = bi;
   __syncthreads();
   for (int h = CURN_RED_THREADS / 2; h > 0; h >>= 1) {
-    if (tid < h && (rv[tid + h] > rv[tid] || (rv[tid + h] == rv[tid] && ri[tid + h] < ri[tid]))) {
+    if (tid < h && fe_better(rv[tid + h], ri[tid + h], rv[tid], ri[tid])) {
       rv[tid] = rv[tid + h];
       ri[tid] = ri[tid + h];
     }
     __syncthreads();
   }
+  // A NaN or +inf maximum makes every e below NaN (NaN - m, inf - inf), and with them every integral; so does an
+  // all -inf map (-inf - -inf), whose ln_bayes is -inf by definition.
   const double mx = rv[0];
-  const int am = ri[0] < n ? ri[0] : 0;
+  const int am = ri[0];
   __syncthreads();   // rv is reused below
   double sk = 0.0;
   if (tid < NA) {
@@ -183,13 +189,14 @@ __global__ void __launch_bounds__(CURN_RED_THREADS) curn_reduce_kernel(const dou
     lmax[r] = mx;
     ml_g[r] = am / NA;
     ml_a[r] = am % NA;
-    lnb[r] = __dadd_rn(mx, log(B));
+    lnb[r] = mx == -INFINITY ? mx : __dadd_rn(mx, log(B));
     const double* x = cm.log10_A;
     double c = 0.0;
     for (int k = 1; k < NA; ++k)
       c = __dadd_rn(c, __dmul_rn(__dmul_rn(0.5, __dsub_rn(x[k], x[k - 1])), __dadd_rn(pa[k - 1], pa[k])));
     const double target = __dmul_rn(cm.ul, c);
-    double lo = 0.0, q = x[NA - 1];
+    // a posterior that is not finite has no quantile: NaN, never the last node (c >= target is false for every NaN)
+    double lo = 0.0, q = isfinite(target) ? x[NA - 1] : NAN;
     c = 0.0;
     for (int k = 1; k < NA; ++k) {
       c = __dadd_rn(c, __dmul_rn(__dmul_rn(0.5, __dsub_rn(x[k], x[k - 1])), __dadd_rn(pa[k - 1], pa[k])));

@@ -46,13 +46,6 @@ __host__ __device__ constexpr size_t fe_smem_bytes(int kp) {
 static_assert(fe_smem_bytes(PTAR_FE_MAX_PSR) <= 227 * 1024, "the Fe tile must fit one SM's shared memory");
 static_assert(PTAR_FE_MAX_PSR % 16 == 0, "kp is a multiple of 16");
 
-// (v, i) ranks above (bv, bi): larger value, then lower index; NaN above every number (the first NaN wins).
-__device__ __forceinline__ bool fe_better(double v, int i, double bv, int bi) {
-  if (v != v) return !(bv != bv) || i < bi;
-  if (bv != bv) return false;
-  return v > bv || (v == bv && i < bi);
-}
-
 // One thread fills stage `st` with sky block `sb`: the antenna block (all kp pulsars x 64 columns) and L4^-1 of (f, sb).
 __device__ __forceinline__ void fe_issue_stage(double* st, uint64_t* bar, const ptar_fe_model& fe, int f, int sb) {
   const uint32_t ab = static_cast<uint32_t>(fe.kp) * FE_BN * 8u, lb = FE_SB * FE_LINV * 8u;

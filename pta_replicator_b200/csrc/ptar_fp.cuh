@@ -180,8 +180,9 @@ __device__ __forceinline__ double fp_q_int(int P, double x) {
   return exp(L) * s;
 }
 
-// One CTA per realization, thread f = frequency: Fp in pulsar order, then (max, first argmax) by a fixed tree; with
-// `fap` also the false-alarm probability Q(n_psr, Fp) per frequency.
+// One CTA per realization, thread f = frequency: Fp in pulsar order, then (max, first argmax) by a fixed tree of
+// fe_better (the first NaN above every number, wherever it sits); with `fap` also the false-alarm probability
+// Q(n_psr, Fp) per frequency (NaN for a NaN Fp, 0 for +inf).
 __global__ void __launch_bounds__(FP_REDUCE_THREADS) fp_reduce_kernel(const double* __restrict__ amps, int nreal,
                                                                       ptar_fp_model fp, double* __restrict__ Fp,
                                                                       double* __restrict__ Fp_max,
@@ -211,7 +212,7 @@ __global__ void __launch_bounds__(FP_REDUCE_THREADS) fp_reduce_kernel(const doub
     if (f < h) {
       const double b = sv[f + h];
       const int bi = si[f + h];
-      if (b > sv[f] || (b == sv[f] && bi < si[f])) {
+      if (fe_better(b, bi, sv[f], si[f])) {
         sv[f] = b;
         si[f] = bi;
       }

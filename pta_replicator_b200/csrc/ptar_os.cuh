@@ -53,6 +53,15 @@ __device__ __forceinline__ void os_mbar_wait(uint64_t* bar, uint32_t parity) {
   }
 }
 
+// The one ranking of every (max, argmax) in the library -- Fp over frequency, Fe over sky and frequency, the radiometer
+// over pixels, ln L over the grid: (v, i) ranks above (bv, bi) on a larger value, then on a lower index; NaN ranks above
+// every number (the first NaN wins).  A total order on (value, index), so a combine is exact whatever its shape.
+__device__ __forceinline__ bool fe_better(double v, int i, double bv, int bi) {
+  if (v != v) return !(bv != bv) || i < bi;
+  if (bv != bv) return false;
+  return v > bv || (v == bv && i < bi);
+}
+
 // Warp 0 fills stage `s` with chunk `c` of the tile: one bulk copy of cnt4 doubles per valid realization row.
 __device__ __forceinline__ void os_issue_chunk(double* stage, uint64_t* bar, const double* rows, int64_t ld, int64_t base,
                                                int nrow, int cnt4, int lane) {

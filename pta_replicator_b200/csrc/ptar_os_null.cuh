@@ -15,7 +15,8 @@
 //                  and the k-half w >> 2 of every 32-kd chunk; the two k-halves are added in a fixed order at the end.
 //                  Every output is therefore summed in an order fixed by kd alone -- not by its r- or s-block, so
 //                  results do not depend on nreal, chunking or real0.  No split-K across CTAs, no atomics.
-// os_null_count    one CTA per realization: #{s >= 1 : S/N_s >= S/N_0} (integer, order-free) and the p-value.
+// os_null_count    one CTA per realization: #{s >= 1 : not S/N_s < S/N_0} (integer, order-free; a NaN null column
+//                  counts) and the p-value (NaN when S/N_0 is NaN).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -165,7 +166,8 @@ __global__ void __launch_bounds__(NL_THREADS) os_null_count_kernel(const double*
   const double* row = snr + r * n_col;
   const double s0 = row[0];
   int c = 0;
-  for (int s = 1 + threadIdx.x; s < n_col; s += NL_THREADS) c += row[s] >= s0;
+  // a NaN null column counts as an exceedance (the conservative side): !(a < b) is a >= b for numbers, true for NaN
+  for (int s = 1 + threadIdx.x; s < n_col; s += NL_THREADS) c += !(row[s] < s0);
   cnt[threadIdx.x] = c;
   __syncthreads();
   for (int h = NL_THREADS / 2; h > 0; h >>= 1) {
@@ -174,7 +176,8 @@ __global__ void __launch_bounds__(NL_THREADS) os_null_count_kernel(const double*
   }
   if (threadIdx.x == 0) {
     exceed[r] = cnt[0];
-    fap[r] = __ddiv_rn(1.0 + cnt[0], static_cast<double>(n_col));
+    // the p-value of a NaN observed S/N is NaN, not the 1 / n_col that zero exceedances would report
+    fap[r] = s0 != s0 ? s0 : __ddiv_rn(1.0 + cnt[0], static_cast<double>(n_col));
   }
 }
 

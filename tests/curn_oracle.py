@@ -76,8 +76,11 @@ def summaries(lnl, log10_A, gamma, kind="log-uniform", ul=0.95):
     am = np.argmax(flat, axis=1)
     m = flat[np.arange(R), am]
     e = np.exp(lnl - m[:, None, None])
-    B = np.einsum("g,k,rgk->r", wg, wx * pi, e)
-    post_a = np.einsum("g,rgk->rk", wg, e) * pi / B[:, None]
+    # B in two stages (gamma, then log10 A): one flat einsum over the NG x NA map accumulates a rounding error of
+    # ~ NG NA u (1e-12 at 256 x 256), more than the summaries it is the yardstick for
+    S = np.einsum("g,rgk->rk", wg, e)
+    B = S @ (wx * pi)
+    post_a = S * pi / B[:, None]
     post_g = np.einsum("k,rgk->rg", wx * pi, e) / B[:, None]
     ulv = np.empty(R)
     for r in range(R):
