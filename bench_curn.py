@@ -15,7 +15,6 @@ nvidia-smi query in the same run.  Writes nothing into the tree.
 """
 from __future__ import annotations
 
-import argparse
 import json
 import os
 import sys
@@ -26,54 +25,17 @@ sys.path.insert(0, ROOT)
 sys.dont_write_bytecode = True   # the tree may be read-only
 
 import bench  # noqa: E402  (the metric workload)
-from bench_postfit import card  # noqa: E402
+from bench_postfit import card, parse, parser, timed_statistic, timing_model_batch  # noqa: E402
 
 
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--steps", type=int, default=5)
-    ap.add_argument("--warmup", type=int, default=3)
-    ap.add_argument("--nreal", type=int, default=1000)
-    ap.add_argument("--kind", default="full", choices=["full", "epoch"])
-    ap.add_argument("--taylor-tol", type=float, default=1e-13)
-    args = ap.parse_args()
-    args.split, args.chunk, args.rc = False, 0, 0
-
-    import numpy as np
-    import torch
-    from pta_replicator_b200 import synthetic
-    torch.cuda.set_device(0)
-    psrs_noise = synthetic.make_ng15_like(args.kind)
-    t0 = time.perf_counter()
-    b, _psrs, _noise, _s, kind = bench.make_batch("2", args, psrs_noise=psrs_noise)
-    for i in range(b.n_psr):
-        b.set_timing_model(i, poly=2, jumps="f")
+    args = parse(parser())
+    b, kind, t0 = timing_model_batch(args)
     b.set_curn_likelihood()
     b.compile()
     setup_s = time.perf_counter() - t0
     R = args.nreal
-
-    def step(k, timers=None):
-        b.curn_likelihood(R, seed=bench.SEED, real0=4 * k * R, timers=timers)
-
-    for k in range(args.warmup):
-        step(k)
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for k in range(args.steps):
-        step(args.warmup + k)
-    e1.record()
-    torch.cuda.synchronize()
-    ms = e0.elapsed_time(e1)
-    timers = {}
-    for k in range(args.steps):
-        step(args.warmup + args.steps + k, timers)
-    torch.cuda.synchronize()
-    per = {}
-    for name, a, z in timers["events"]:
-        per.setdefault(name, []).append(a.elapsed_time(z))
-    kms = {k: float(np.sum(v)) / args.steps for k, v in per.items()}
+    ms, kms = timed_statistic(b.curn_likelihood, R, args.steps, args.warmup)
     st = b.compile()["curn"]
     m = st["curn"]
     flop = 2.0 * R * m.n_gamma * b.n_psr * m.nc * (m.nc + m.n_amp)

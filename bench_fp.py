@@ -16,7 +16,6 @@ name and power limit are read with a read-only nvidia-smi query in the same run.
 """
 from __future__ import annotations
 
-import argparse
 import json
 import os
 import sys
@@ -27,58 +26,23 @@ sys.path.insert(0, ROOT)
 sys.dont_write_bytecode = True   # the tree may be read-only
 
 import bench  # noqa: E402  (the metric workload)
-from bench_postfit import card  # noqa: E402
+from bench_postfit import card, parse, parser, timed_statistic, timing_model_batch  # noqa: E402
 
 FP64_TC_PEAK = 67.0   # TFLOP/s, H100 SXM data sheet (not measured)
 
 
 def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--steps", type=int, default=5)
-    ap.add_argument("--warmup", type=int, default=3)
-    ap.add_argument("--nreal", type=int, default=1000)
-    ap.add_argument("--kind", default="full", choices=["full", "epoch"])
-    ap.add_argument("--taylor-tol", type=float, default=1e-13)
+    ap = parser()
     ap.add_argument("--n-freqs", type=int, default=100)
-    args = ap.parse_args()
-    args.split, args.chunk, args.rc = False, 0, 0
+    args = parse(ap)
 
-    import numpy as np
-    import torch
-    from pta_replicator_b200 import synthetic
-    torch.cuda.set_device(0)
-    psrs_noise = synthetic.make_ng15_like(args.kind)
-    t0 = time.perf_counter()
-    b, _psrs, _noise, _s, kind = bench.make_batch("2", args, psrs_noise=psrs_noise)
-    for i in range(b.n_psr):
-        b.set_timing_model(i, poly=2, jumps="f")
+    b, kind, t0 = timing_model_batch(args)
     gw_log10_A = -14.6733                                   # the GWB amplitude config 2 injects (synthetic.ng15_recipe)
     b.set_fp_statistic(n_freqs=args.n_freqs, log10_A_common=gw_log10_A)
     st = b.compile()["fp"]
     setup_s = time.perf_counter() - t0
     R = args.nreal
-
-    def step(k, timers=None):
-        b.fp_statistic(R, seed=bench.SEED, real0=4 * k * R, timers=timers)
-
-    for k in range(args.warmup):
-        step(k)
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for k in range(args.steps):
-        step(args.warmup + k)
-    e1.record()
-    torch.cuda.synchronize()
-    ms = e0.elapsed_time(e1)
-    timers = {}
-    for k in range(args.steps):
-        step(args.warmup + args.steps + k, timers)
-    torch.cuda.synchronize()
-    per = {}
-    for name, a, z in timers["events"]:
-        per.setdefault(name, []).append(a.elapsed_time(z))
-    kms = {k: float(np.sum(v)) / args.steps for k, v in per.items()}
+    ms, kms = timed_statistic(b.fp_statistic, R, args.steps, args.warmup)
     flop = 2.0 * R * b.n_toa_total * 2 * args.n_freqs
     tflops = flop / (kms["fp_project"] * 1e-3) / 1e12
     line = {"metric": "realizations/sec of fp_statistic (67-psr ng15 GWB+RN+ECORR, spin + JUMPs marginalised)",

@@ -37,27 +37,75 @@ def card():
         return None
 
 
-def main():
+def parser():
+    """The options of every benchmark on the timing-model workload (this one and the statistic benchmarks)."""
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--nreal", type=int, default=1000)
     ap.add_argument("--kind", default="full", choices=["full", "epoch"])
-    ap.add_argument("--rc", type=int, default=0)
-    ap.add_argument("--chunk", type=int, default=0)
     ap.add_argument("--taylor-tol", type=float, default=1e-13)
-    args = ap.parse_args()
-    args.split = False
+    return ap
 
+
+def parse(ap):
+    """``ap``'s arguments; bench.make_batch's split, chunk and rc are off unless ``ap`` has an option for them."""
+    return ap.parse_args(namespace=argparse.Namespace(split=False, chunk=0, rc=0))
+
+
+def timing_model_batch(args):
+    """bench.py's config-2 batch on device 0 with ``set_timing_model(i, poly=2, jumps="f")`` on every pulsar.  Returns
+    (batch, kind, t0) with t0 the perf_counter reading after the pulsars are made and before the batch is built: the
+    caller's setup clock, stopped after its own registrations and ``compile()``."""
     import torch
     from pta_replicator_b200 import synthetic
     torch.cuda.set_device(0)
-    hbm, how = bench.peaks()
     psrs_noise = synthetic.make_ng15_like(args.kind)
     t0 = time.perf_counter()
     b, _psrs, _noise, _s, kind = bench.make_batch("2", args, psrs_noise=psrs_noise)
     for i in range(b.n_psr):
         b.set_timing_model(i, poly=2, jumps="f")
+    return b, kind, t0
+
+
+def timed_statistic(fn, R, steps, warmup):
+    """Time ``fn(R, seed, real0, timers)`` (a statistic of R generated realizations): ``warmup`` untimed calls, ``steps``
+    calls between two CUDA events, then ``steps`` more with per-launch timers.  Every call draws fresh realizations.
+    Returns (ms of the event-timed calls, {kernel: ms per step} of the timed-launch pass)."""
+    import numpy as np
+    import torch
+
+    def step(k, timers=None):
+        fn(R, seed=bench.SEED, real0=4 * k * R, timers=timers)
+
+    for k in range(warmup):
+        step(k)
+    torch.cuda.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for k in range(steps):
+        step(warmup + k)
+    e1.record()
+    torch.cuda.synchronize()
+    ms = e0.elapsed_time(e1)
+    timers = {}
+    for k in range(steps):
+        step(warmup + steps + k, timers)
+    torch.cuda.synchronize()
+    per = {}
+    for name, a, z in timers["events"]:
+        per.setdefault(name, []).append(a.elapsed_time(z))
+    return ms, {k: float(np.sum(v)) / steps for k, v in per.items()}
+
+
+def main():
+    ap = parser()
+    ap.add_argument("--rc", type=int, default=0)
+    ap.add_argument("--chunk", type=int, default=0)
+    args = parse(ap)
+
+    hbm, how = bench.peaks()
+    b, kind, t0 = timing_model_batch(args)
     tm = b.plan()["tm"]
     b.compile()
     setup_s = time.perf_counter() - t0

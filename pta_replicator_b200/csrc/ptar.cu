@@ -630,13 +630,18 @@ int ptar_timing_project(double* out, int64_t ld_out, int32_t nreal, const ptar_t
   return ptar_timing_project_stage(out, ld_out, nreal, tm, scratch, scratch_len, 0, stream);
 }
 
+// The basis width of the projection X [nreal][n_psr][ncp] (0 < nc <= 32, ncp = nc rounded up to a multiple of 8) and
+// the (log10 A, gamma) grid of the CURN and HD likelihoods (2 <= n_amp <= 256, 1 <= n_gamma <= 256).
+static inline bool nc_ok(int32_t nc, int32_t ncp) { return nc > 0 && nc <= PTAR_OS_MAX_NC && ncp == ((nc + 7) & ~7); }
+static inline bool grid_ok(int32_t na, int32_t ng) { return na >= 2 && na <= PTAR_CURN_MAX_NA && ng >= 1 && ng <= PTAR_CURN_MAX_NG; }
+
 int ptar_os_project_stage(const double* rows, int64_t ld, int32_t nreal, const ptar_os_model* os, double* partial,
                           int64_t partial_len, double* X, int stage, void* stream) {
   if (!rows || !os || !partial || !X || nreal <= 0 || ld <= 0 || stage < 0 || stage > 2)
     return fail(-1, "ptar_os_project: bad argument%s");
   if (!os->tiles || !os->tile0 || !os->n_tile || !os->C || os->n_tiles <= 0 || os->n_psr <= 0)
     return fail(-2, "ptar_os_project: model arrays missing%s");
-  if (os->nc <= 0 || os->nc > PTAR_OS_MAX_NC || os->ncp != ((os->nc + 7) & ~7))
+  if (!nc_ok(os->nc, os->ncp))
     return fail(-2, "ptar_os_project: need 0 < nc <= 32 and ncp = nc rounded up to a multiple of 8%s");
   if ((ld & 3) || (reinterpret_cast<uintptr_t>(rows) & 31))
     return fail(-2, "ptar_os_project: rows must be 32-byte aligned with ld %% 4 == 0%s");
@@ -683,7 +688,7 @@ int ptar_os_pairs(const double* X, int32_t nreal, const ptar_os_model* os, doubl
   if (os->n_psr < 2 || os->n_psr > PTAR_OS_MAX_PSR) return fail(-3, "ptar_os_pairs: need 2..256 pulsars%s");
   if (os->n_orf <= 0 || os->n_orf > PTAR_OS_MAX_ORF || os->n_pairs <= 0)
     return fail(-2, "ptar_os_pairs: need 1..4 templates and at least one pair%s");
-  if (os->nc <= 0 || os->nc > PTAR_OS_MAX_NC || os->ncp != ((os->nc + 7) & ~7))
+  if (!nc_ok(os->nc, os->ncp))
     return fail(-2, "ptar_os_pairs: need 0 < nc <= 32 and ncp = nc rounded up to a multiple of 8%s");
   const size_t smem = sizeof(double) * (size_t(os->n_psr) * os->ncp + size_t(PTAR_OS_MAX_ORF) * ptar::OS_PAIR_THREADS);
   static SmemOptIn optin;
@@ -696,6 +701,30 @@ int ptar_os_pairs(const double* X, int32_t nreal, const ptar_os_model* os, doubl
   return check_launch("ptar_os_pairs");
 }
 
+// Stages 1 and 2 (0: both) of ptar_os_null and ptar_os_aniso: the pair products U of X (os_null_prepare_kernel), then
+// out = U V / dsqrt over the column set of nl (os_null_gemm_kernel).  Errors name the entry point ``what`` and the stage.
+static int os_pair_gemm(const double* X, int32_t nreal, const ptar_os_model& os, const ptar_os_null_model& nl, double* U,
+                        double* out, int stage, cudaStream_t st, const char* what) {
+  char msg[64];
+  if (stage == 0 || stage == 1) {
+    snprintf(msg, sizeof(msg), "%s (prepare)", what);
+    static SmemOptIn optin;
+    if (int rc = opt_in_smem(ptar::os_null_prepare_kernel, optin, sizeof(double) * PTAR_OS_MAX_PSR * PTAR_OS_MAX_NC, msg)) return rc;
+    const size_t smem = sizeof(double) * size_t(os.n_psr) * os.ncp;
+    ptar::os_null_prepare_kernel<<<static_cast<unsigned>(nreal), ptar::NL_THREADS, smem, st>>>(X, os, nl, U);
+    if (int rc = check_launch(msg)) return rc;
+  }
+  if (stage == 0 || stage == 2) {
+    snprintf(msg, sizeof(msg), "%s (GEMM)", what);
+    static SmemOptIn optin;
+    if (int rc = opt_in_smem(ptar::os_null_gemm_kernel, optin, ptar::NL_SMEM, msg)) return rc;
+    const dim3 grid(static_cast<unsigned>(nl.n_colp / ptar::NL_BN), static_cast<unsigned>((nreal + ptar::NL_BM - 1) / ptar::NL_BM));
+    ptar::os_null_gemm_kernel<<<grid, ptar::NL_THREADS, ptar::NL_SMEM, st>>>(U, nreal, nl, out);
+    if (int rc = check_launch(msg)) return rc;
+  }
+  return 0;
+}
+
 int ptar_os_null_stage(const double* X, int32_t nreal, const ptar_os_model* os, const ptar_os_null_model* nl, double* U,
                        double* snr, int64_t* exceed, double* fap, int stage, void* stream) {
   if (!X || !os || !nl || !U || !snr || !exceed || !fap || nreal <= 0 || stage < 0 || stage > 3)
@@ -703,7 +732,7 @@ int ptar_os_null_stage(const double* X, int32_t nreal, const ptar_os_model* os, 
   if (!os->sqrt_phi || !os->pairs || !nl->V || !nl->dsqrt) return fail(-2, "ptar_os_null: model arrays missing%s");
   if (os->n_psr < 2 || os->n_psr > PTAR_OS_MAX_PSR || os->n_pairs != os->n_psr * (os->n_psr - 1) / 2)
     return fail(-3, "ptar_os_null: need 2..256 pulsars and every pair%s");
-  if (os->nc <= 0 || os->nc > PTAR_OS_MAX_NC || (os->nc & 1) || os->ncp != ((os->nc + 7) & ~7))
+  if (!nc_ok(os->nc, os->ncp) || (os->nc & 1))
     return fail(-2, "ptar_os_null: need an even 0 < nc <= 32 and ncp = nc rounded up to a multiple of 8%s");
   if (nl->method != PTAR_OS_NULL_PHASE_SHIFT && nl->method != PTAR_OS_NULL_SKY_SCRAMBLE)
     return fail(-2, "ptar_os_null: unknown method%s");
@@ -713,22 +742,7 @@ int ptar_os_null_stage(const double* X, int32_t nreal, const ptar_os_model* os, 
   if (nl->kd != kd || nl->kdp != ((kd + ptar::NL_BK - 1) & ~int64_t(ptar::NL_BK - 1)))
     return fail(-2, "ptar_os_null: kd must be 2 K n_pairs (phase shift) or n_pairs (sky scramble), kdp kd rounded up to 32%s");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (stage == 0 || stage == 1) {
-    const size_t smem = sizeof(double) * size_t(os->n_psr) * os->ncp;
-    static SmemOptIn optin;
-    if (int rc = opt_in_smem(ptar::os_null_prepare_kernel, optin, sizeof(double) * size_t(PTAR_OS_MAX_PSR) * PTAR_OS_MAX_NC,
-                             "ptar_os_null (prepare)"))
-      return rc;
-    ptar::os_null_prepare_kernel<<<static_cast<unsigned>(nreal), ptar::NL_THREADS, smem, st>>>(X, *os, *nl, U);
-    if (int rc = check_launch("ptar_os_null (prepare)")) return rc;
-  }
-  if (stage == 0 || stage == 2) {
-    static SmemOptIn optin;
-    if (int rc = opt_in_smem(ptar::os_null_gemm_kernel, optin, ptar::NL_SMEM, "ptar_os_null (GEMM)")) return rc;
-    const dim3 grid(static_cast<unsigned>(nl->n_colp / ptar::NL_BN), static_cast<unsigned>((nreal + ptar::NL_BM - 1) / ptar::NL_BM));
-    ptar::os_null_gemm_kernel<<<grid, ptar::NL_THREADS, ptar::NL_SMEM, st>>>(U, nreal, *nl, snr);
-    if (int rc = check_launch("ptar_os_null (GEMM)")) return rc;
-  }
+  if (int rc = os_pair_gemm(X, nreal, *os, *nl, U, snr, stage, st, "ptar_os_null")) return rc;
   if (stage == 0 || stage == 3) {
     ptar::os_null_count_kernel<<<static_cast<unsigned>(nreal), ptar::NL_THREADS, 0, st>>>(snr, nl->n_col, exceed, fap);
     if (int rc = check_launch("ptar_os_null (count)")) return rc;
@@ -748,7 +762,7 @@ int ptar_os_aniso_stage(const double* X, int32_t nreal, const ptar_os_model* os,
   if (!os->sqrt_phi || !os->pairs || !am->V || !am->dsqrt) return fail(-2, "ptar_os_aniso: model arrays missing%s");
   if (os->n_psr < 2 || os->n_psr > PTAR_OS_MAX_PSR || os->n_pairs != os->n_psr * (os->n_psr - 1) / 2)
     return fail(-3, "ptar_os_aniso: need 2..256 pulsars and every pair%s");
-  if (os->nc <= 0 || os->nc > PTAR_OS_MAX_NC || os->ncp != ((os->nc + 7) & ~7))
+  if (!nc_ok(os->nc, os->ncp))
     return fail(-2, "ptar_os_aniso: need 0 < nc <= 32 and ncp = nc rounded up to a multiple of 8%s");
   if (am->n_lm < 0 || am->n_lm > PTAR_OS_ANISO_MAX_LM || am->n_z != std::max(am->n_lm - 1, 0) || am->n_sky < 0 ||
       am->n_sky > PTAR_OS_ANISO_MAX_SKY || am->n_lm + am->n_sky < 1)
@@ -762,22 +776,7 @@ int ptar_os_aniso_stage(const double* X, int32_t nreal, const ptar_os_model* os,
   // the sky-scramble operands of ptar_os_null: U[r][q] = x_a . x_b, V^T rows = the columns of the anisotropy map
   const ptar_os_null_model nl{PTAR_OS_NULL_SKY_SCRAMBLE, am->n_col, am->n_colp, 0, am->kd, am->kdp, am->V, am->dsqrt};
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (stage == 0 || stage == 1) {
-    const size_t smem = sizeof(double) * size_t(os->n_psr) * os->ncp;
-    static SmemOptIn optin;
-    if (int rc = opt_in_smem(ptar::os_null_prepare_kernel, optin, sizeof(double) * size_t(PTAR_OS_MAX_PSR) * PTAR_OS_MAX_NC,
-                             "ptar_os_aniso (prepare)"))
-      return rc;
-    ptar::os_null_prepare_kernel<<<static_cast<unsigned>(nreal), ptar::NL_THREADS, smem, st>>>(X, *os, nl, U);
-    if (int rc = check_launch("ptar_os_aniso (prepare)")) return rc;
-  }
-  if (stage == 0 || stage == 2) {
-    static SmemOptIn optin;
-    if (int rc = opt_in_smem(ptar::os_null_gemm_kernel, optin, ptar::NL_SMEM, "ptar_os_aniso (GEMM)")) return rc;
-    const dim3 grid(static_cast<unsigned>(nl.n_colp / ptar::NL_BN), static_cast<unsigned>((nreal + ptar::NL_BM - 1) / ptar::NL_BM));
-    ptar::os_null_gemm_kernel<<<grid, ptar::NL_THREADS, ptar::NL_SMEM, st>>>(U, nreal, nl, map);
-    if (int rc = check_launch("ptar_os_aniso (GEMM)")) return rc;
-  }
+  if (int rc = os_pair_gemm(X, nreal, *os, nl, U, map, stage, st, "ptar_os_aniso")) return rc;
   if (stage == 0 || stage == 3) {
     ptar::os_aniso_reduce_kernel<<<static_cast<unsigned>(nreal), ptar::AN_THREADS, 0, st>>>(map, *am, clm, z, chi2, snr_max,
                                                                                           argmax, radio_map);
@@ -868,9 +867,9 @@ int ptar_fe_combine(const double* fmax, const int64_t* fargmax, int32_t nreal, c
 static int curn_model_check(const ptar_curn_model* cm, const char* what) {
   if (!cm->V || !cm->lam || !cm->a2 || !cm->ldet || !cm->log10_A || !cm->wg || !cm->wx || !cm->prior || cm->n_psr <= 0)
     return fail(-2, "%s: model arrays missing", what);
-  if (cm->nc <= 0 || cm->nc > PTAR_OS_MAX_NC || cm->ncp != ((cm->nc + 7) & ~7))
+  if (!nc_ok(cm->nc, cm->ncp))
     return fail(-2, "%s: need 0 < nc <= 32 and ncp = nc rounded up to a multiple of 8", what);
-  if (cm->n_amp < 2 || cm->n_amp > PTAR_CURN_MAX_NA || cm->n_gamma < 1 || cm->n_gamma > PTAR_CURN_MAX_NG)
+  if (!grid_ok(cm->n_amp, cm->n_gamma))
     return fail(-2, "%s: need 2 <= n_amp <= 256 and 1 <= n_gamma <= 256", what);
   if (!(cm->ul > 0.0 && cm->ul < 1.0)) return fail(-2, "%s: need 0 < ul < 1", what);
   return 0;
@@ -916,12 +915,12 @@ int ptar_curn_reduce(const double* lnL, int32_t nreal, const ptar_curn_model* cm
 int ptar_hd_grid(const double* X, int32_t nreal, const ptar_hd_model* hm, double* lnL, void* stream) {
   if (!X || !hm || !lnL || nreal <= 0) return fail(-1, "ptar_hd_grid: bad argument%s");
   if (!hm->V || !hm->lam || !hm->a2 || !hm->ldet || hm->n_psr <= 0) return fail(-2, "ptar_hd_grid: model arrays missing%s");
-  if (hm->nc <= 0 || hm->nc > PTAR_OS_MAX_NC || hm->ncp != ((hm->nc + 7) & ~7))
+  if (!nc_ok(hm->nc, hm->ncp))
     return fail(-2, "ptar_hd_grid: need 0 < nc <= 32 and ncp = nc rounded up to a multiple of 8%s");
   if (int64_t(hm->n) != int64_t(hm->n_psr) * hm->nc || hm->n > PTAR_HD_MAX_N ||
       hm->np != (hm->n + PTAR_HD_JB - 1) / PTAR_HD_JB * PTAR_HD_JB)
     return fail(-2, "ptar_hd_grid: need n = n_psr nc <= 4096 and np = n rounded up to a multiple of 32%s");
-  if (hm->n_amp < 2 || hm->n_amp > PTAR_CURN_MAX_NA || hm->n_gamma < 1 || hm->n_gamma > PTAR_CURN_MAX_NG)
+  if (!grid_ok(hm->n_amp, hm->n_gamma))
     return fail(-2, "ptar_hd_grid: need 2 <= n_amp <= 256 and 1 <= n_gamma <= 256%s");
   if ((reinterpret_cast<uintptr_t>(X) & 31) || (reinterpret_cast<uintptr_t>(hm->V) & 15))
     return fail(-2, "ptar_hd_grid: X must be 32-byte aligned, V 16-byte aligned%s");
