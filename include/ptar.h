@@ -46,6 +46,7 @@
  *   ptar_os_pairs          device instead of gathering the rows
  *   ptar_os_null           no counterpart: phase-shift / sky-scramble null distribution and p-value per realization
  *   ptar_os_aniso          no counterpart: spherical-harmonic fit, anisotropy chi^2 and radiometer sky map per realization
+ *   ptar_os_pf             no counterpart: per-frequency optimal statistic (GW power at every f_k) per realization
  *   ptar_fp_project /      no counterpart: the incoherent Fp-statistic of continuous waves per realization and search
  *   ptar_fp_reduce         frequency, reduced on the device
  *   ptar_curn_grid /       no counterpart (an MCMC over enterprise's CURN model per realization): the common-process
@@ -67,7 +68,8 @@ extern "C" {
                              (ptar_timing_model, ptar_timing_project[_stage], ptar_run_job[_to_host]_tm) and the optimal
                              statistic (ptar_os_model, ptar_os_project[_stage], ptar_os_pairs), its null distributions
                              (ptar_os_null_model, ptar_os_null[_stage]) and anisotropy (ptar_os_aniso_model,
-                             ptar_os_aniso[_stage], PTAR_OS_ANISO_MAX_LM / _SKY), the Fp-statistic (ptar_fp_model,
+                             ptar_os_aniso[_stage], PTAR_OS_ANISO_MAX_LM / _SKY) and per-frequency form
+                             (ptar_os_pf_model, ptar_os_pf), the Fp-statistic (ptar_fp_model,
                              ptar_fp_project, ptar_fp_reduce[_fap], PTAR_FP_MAX_FREQ), the CURN likelihood
                              (ptar_curn_model, ptar_curn_grid, ptar_curn_reduce, PTAR_CURN_MAX_NA / _NG) and the HD
                              likelihood (ptar_hd_model, ptar_hd_grid, PTAR_HD_MAX_N / _JB) are new symbols only, so a
@@ -409,6 +411,25 @@ int ptar_os_aniso(const double* X, int32_t nreal, const ptar_os_model* os, const
 int ptar_os_aniso_stage(const double* X, int32_t nreal, const ptar_os_model* os, const ptar_os_aniso_model* model,
                         double* U, double* map, double* clm, double* z, double* chi2, double* snr_max, int64_t* argmax,
                         double* radio_map, int stage, void* stream);
+
+/* Per-frequency optimal statistic (csrc/ptar_os_pf.cuh), from statics derived once on the host.  K = nc / 2 GW
+ * frequencies f_k; Z_a[k] is the 2 x 2 diagonal block of Z_a at frequency k.  Per realization r, from the unscaled X of
+ * ptar_os_project (no phi~ factor), frequency k, pair q = (a, b) of os and template o:
+ *   d_qk = X_a,2k X_b,2k + X_a,2k+1 X_b,2k+1;  rho[r][k][q] = d_qk / t[k][q]  (rho may be NULL);
+ *   b_ok = sum_q orf[o][q] d_qk;  phi[r][o][k] = b_ok / dnorm[o][k];  snr[r][o][k] = b_ok / dsqrt[o][k];
+ *   phi_mc[r][o][k] = sum_o' finv[k][o][o'] b_o'k.
+ * One launch.  Each sum runs in an order fixed by q and k only: outputs are bit-identical whatever nreal, chunking or
+ * real0. */
+typedef struct {
+  const double* t;          /* [K][n_pairs] t_qk = tr(Z_a[k] Z_b[k])                                              */
+  const double* dnorm;      /* [n_orf][K] D_ok = sum_q Gamma^o_q^2 t_qk                                           */
+  const double* dsqrt;      /* [n_orf][K] sqrt(D_ok)                                                              */
+  const double* finv;       /* [K][n_orf][n_orf] F_k^{-1}, (F_k)_oo' = sum_q Gamma^o_q Gamma^o'_q t_qk             */
+} ptar_os_pf_model;
+
+/* rho: [nreal][K][n_pairs] or NULL; phi, snr, phi_mc: [nreal][n_orf][K].  X as for ptar_os_pairs; os->nc even. */
+int ptar_os_pf(const double* X, int32_t nreal, const ptar_os_model* os, const ptar_os_pf_model* pf, double* rho,
+               double* phi, double* snr, double* phi_mc, void* stream);
 
 /* Incoherent Fp-statistic (csrc/ptar_fp.cuh).  The host derives, once per recipe, for every pulsar a and search
  * frequency f the whitened basis C~_a(f) = P_a^{-1} F_f L_a(f)^{-T} (F_f = (sin, cos)(2 pi f t), P_a the noise

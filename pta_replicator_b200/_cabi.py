@@ -50,7 +50,7 @@ EXPORTS = ("ptar_version", "ptar_last_error", "ptar_cholesky_lower", "ptar_fouri
            "ptar_gwb_mix", "ptar_gwb_synth", "ptar_gwb_mix_i8", "ptar_gwb_slice_i8", "ptar_gwb_synth_i8", "ptar_debug_i8_timestamps", "ptar_generate", "ptar_generate_stage", "ptar_philox_normals", "ptar_peer_export", "ptar_peer_open", "ptar_peer_close", "ptar_peer_copy", "ptar_run_job",
            "ptar_run_job_to_host", "ptar_timing_project", "ptar_timing_project_stage",
            "ptar_run_job_tm", "ptar_run_job_to_host_tm", "ptar_os_project", "ptar_os_project_stage", "ptar_os_pairs",
-           "ptar_os_null", "ptar_os_null_stage", "ptar_os_aniso", "ptar_os_aniso_stage", "ptar_fp_project", "ptar_fp_reduce",
+           "ptar_os_null", "ptar_os_null_stage", "ptar_os_aniso", "ptar_os_aniso_stage", "ptar_os_pf", "ptar_fp_project", "ptar_fp_reduce",
            "ptar_fp_reduce_fap", "ptar_fe_sky", "ptar_fe_combine", "ptar_curn_grid", "ptar_curn_reduce",
            "ptar_hd_grid")
 OS_MAX_NC, OS_MAX_ORF, OS_MAX_PSR = 32, 4, 256     # optimal statistic: GW-basis columns, templates, pulsars (ptar.h)
@@ -119,6 +119,10 @@ class OsAnisoModel(C.Structure):
     _fields_ = [("n_lm", C.c_int32), ("n_z", C.c_int32), ("n_sky", C.c_int32), ("n_col", C.c_int32),
                 ("n_colp", C.c_int32), ("reserved", C.c_int32), ("kd", C.c_int64), ("kdp", C.c_int64), ("V", C.c_void_p),
                 ("dsqrt", C.c_void_p)]
+
+
+class OsPfModel(C.Structure):
+    _fields_ = [("t", C.c_void_p), ("dnorm", C.c_void_p), ("dsqrt", C.c_void_p), ("finv", C.c_void_p)]
 
 
 class FpModel(C.Structure):
@@ -196,6 +200,7 @@ def lib():
     L.ptar_os_null_stage.argtypes = [vp, C.c_int32, vp, vp, vp, vp, vp, vp, i32, vp]
     L.ptar_os_aniso.argtypes = [vp, C.c_int32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]   # model: an OsAnisoModel
     L.ptar_os_aniso_stage.argtypes = [vp, C.c_int32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, vp]
+    L.ptar_os_pf.argtypes = [vp, C.c_int32, vp, vp, vp, vp, vp, vp, vp]                  # pf: address of an OsPfModel
     L.ptar_fp_project.argtypes = [vp, i64, C.c_int32, vp, vp, vp]                        # fp: address of an FpModel
     L.ptar_fp_reduce.argtypes = [vp, C.c_int32, vp, vp, vp, vp, vp]
     L.ptar_fp_reduce_fap.argtypes = [vp, C.c_int32, vp, vp, vp, vp, vp, vp]

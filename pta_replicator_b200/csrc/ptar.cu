@@ -19,6 +19,7 @@
 #include "ptar_os.cuh"
 #include "ptar_os_aniso.cuh"
 #include "ptar_os_null.cuh"
+#include "ptar_os_pf.cuh"
 #include "ptar_rng.cuh"
 #include "ptar_timing.cuh"
 
@@ -699,6 +700,25 @@ int ptar_os_pairs(const double* X, int32_t nreal, const ptar_os_model* os, doubl
   ptar::os_pairs_kernel<<<static_cast<unsigned>(nreal), ptar::OS_PAIR_THREADS, smem, static_cast<cudaStream_t>(stream)>>>(
       X, nreal, *os, rho, a2, snr, a2_mc);
   return check_launch("ptar_os_pairs");
+}
+
+int ptar_os_pf(const double* X, int32_t nreal, const ptar_os_model* os, const ptar_os_pf_model* pf, double* rho,
+               double* phi, double* snr, double* phi_mc, void* stream) {
+  if (!X || !os || !pf || !phi || !snr || !phi_mc || nreal <= 0) return fail(-1, "ptar_os_pf: bad argument%s");
+  if (!os->pairs || !os->orf || !pf->t || !pf->dnorm || !pf->dsqrt || !pf->finv)
+    return fail(-2, "ptar_os_pf: model arrays missing%s");
+  if (os->n_psr < 2 || os->n_psr > PTAR_OS_MAX_PSR) return fail(-3, "ptar_os_pf: need 2..256 pulsars%s");
+  if (os->n_orf <= 0 || os->n_orf > PTAR_OS_MAX_ORF || os->n_pairs <= 0)
+    return fail(-2, "ptar_os_pf: need 1..4 templates and at least one pair%s");
+  if (!nc_ok(os->nc, os->ncp) || (os->nc & 1))
+    return fail(-2, "ptar_os_pf: need an even 0 < nc <= 32 and ncp = nc rounded up to a multiple of 8%s");
+  const size_t smem = sizeof(double) * size_t(os->n_psr) * os->nc;
+  static SmemOptIn optin;
+  if (int rc = opt_in_smem(ptar::os_pf_kernel, optin, sizeof(double) * size_t(PTAR_OS_MAX_PSR) * PTAR_OS_MAX_NC, "ptar_os_pf"))
+    return rc;
+  ptar::os_pf_kernel<<<static_cast<unsigned>(nreal), ptar::PF_THREADS, smem, static_cast<cudaStream_t>(stream)>>>(
+      X, *os, *pf, rho, phi, snr, phi_mc);
+  return check_launch("ptar_os_pf");
 }
 
 // Stages 1 and 2 (0: both) of ptar_os_null and ptar_os_aniso: the pair products U of X (os_null_prepare_kernel), then
