@@ -53,6 +53,8 @@
  *   ptar_curn_reduce       likelihood on an (A, gamma) grid, its maximum, Bayes factor, marginals and upper limit
  *   ptar_hd_grid           no counterpart (an MCMC over enterprise's HD-correlated model per realization): the
  *                          ORF-correlated common-process likelihood on the CURN grid, reduced by ptar_curn_reduce
+ *   ptar_rn_grid           no counterpart (a single-pulsar noise analysis per realization and pulsar): each pulsar's
+ *                          intrinsic red-noise likelihood on an (A, gamma) grid, reduced by ptar_curn_reduce
  */
 #ifndef PTAR_H
 #define PTAR_H
@@ -72,8 +74,10 @@ extern "C" {
                              (ptar_os_pf_model, ptar_os_pf), the Fp-statistic (ptar_fp_model,
                              ptar_fp_project, ptar_fp_reduce[_fap], PTAR_FP_MAX_FREQ), the CURN likelihood
                              (ptar_curn_model, ptar_curn_grid, ptar_curn_reduce, PTAR_CURN_MAX_NA / _NG) and the HD
-                             likelihood (ptar_hd_model, ptar_hd_grid, PTAR_HD_MAX_N / _JB) are new symbols only, so a
-                             caller detects them by looking the symbol up. */
+                             likelihood (ptar_hd_model, ptar_hd_grid, PTAR_HD_MAX_N / _JB) and the single-pulsar
+                             red-noise likelihood (ptar_rn_model, ptar_rn_grid, PTAR_RN_MAX_NC) are new symbols only, so
+                             a caller detects them by looking the symbol up.  ptar_os_project accepts nc up to
+                             PTAR_RN_MAX_NC since the red-noise likelihood; nothing changes for nc <= PTAR_OS_MAX_NC. */
 
 /* Geometry limits of the fused generator kernel. */
 #define PTAR_TILE_TOAS   1024  /* TOAs per tile (256 threads x 4)            */
@@ -308,8 +312,11 @@ int ptar_timing_project_stage(double* out, int64_t ld_out, int32_t nreal, const 
  *                    a2[r][o] = b_o / dnorm[o];  snr[r][o] = b_o / dsqrt[o];  a2_mc[r][o] = sum_o' finv[o][o'] b_o'.
  * Every sum runs in an order fixed by the tile, the TOA index and the pair list only: outputs are bit-identical
  * whatever nreal, chunking, real0 or launch grid produced the rows.  ptar_os_project_stage runs one of the two
- * launches of ptar_os_project (stage 1 = tile GEMM, 2 = tile sums) so a caller can time them. */
+ * launches of ptar_os_project (stage 1 = tile GEMM, 2 = tile sums) so a caller can time them.  ptar_os_project alone
+ * takes nc up to PTAR_RN_MAX_NC (the red-noise likelihood's bases); every other entry point of a ptar_os_model needs
+ * nc <= PTAR_OS_MAX_NC. */
 #define PTAR_OS_MAX_NC  32    /* GW-basis columns (2K)                 */
+#define PTAR_RN_MAX_NC  64    /* basis columns of ptar_os_project and ptar_rn_grid (2 x 32 red-noise components) */
 #define PTAR_OS_MAX_ORF 4     /* templates                             */
 #define PTAR_OS_MAX_PSR 256   /* pulsars (pair kernel: x in shared memory) */
 typedef struct {
@@ -575,6 +582,34 @@ typedef struct {
 
 /* lnL: [nreal][n_gamma][n_amp]. */
 int ptar_hd_grid(const double* X, int32_t nreal, const ptar_hd_model* hm, double* lnL, void* stream);
+
+/* Single-pulsar intrinsic red-noise likelihood on an (A, gamma) grid (csrc/ptar_rn.cuh), from the X of ptar_os_project
+ * run on each pulsar's own red-noise basis F_a (f_k = k / T_a, nc = 2K <= PTAR_RN_MAX_NC).  The host derives, once per
+ * recipe, for every pulsar a and grid gamma the eigendecomposition phi~_a^{1/2} Z_a phi~_a^{1/2} = U diag(lambda) U^T
+ * (Z_a = F_a^T P_a^{-1} F_a, P_a without the pulsar's own red noise, phi~_a the power law at A = 1, gamma and T_a),
+ * V_a(gamma) = U^T phi~_a^{1/2} and ldet[a][g][k] = sum_j log1p(A_k^2 lambda_j).  Per realization r:
+ *   ptar_rn_grid  lnL[r][a][g][k] = 1/2 sum_j w_j y_j^2 - 1/2 ldet[a][g][k],  y = V_a(gamma_g) X[r][a],
+ *                 w_j = A_k^2 / (1 + A_k^2 lambda_j): two chained GEMMs on the fp64 tensor cores, no sum over pulsars.
+ *                 X: [nreal][n_psr][ncp], 32-byte aligned.
+ * The summaries of the nreal * n_psr maps [r][a] are ptar_curn_reduce's, called with nreal * n_psr and a
+ * ptar_curn_model carrying the grid (log10_A, wg, wx, prior, ul, n_amp, n_gamma).  Outputs are bit-identical whatever
+ * nreal, chunking or real0. */
+typedef struct {
+  int32_t n_psr;              /* n_psr * ceil(n_gamma / 16) <= 65535                                               */
+  int32_t nc;                 /* 2K <= PTAR_RN_MAX_NC                                                              */
+  int32_t ncp;                /* nc rounded up to a multiple of 8 (as the ptar_os_model of the projection)         */
+  int32_t n_gamma;            /* 1 .. PTAR_CURN_MAX_NG                                                             */
+  int32_t n_amp;              /* 2 .. PTAR_CURN_MAX_NA                                                             */
+  int32_t reserved;
+  const double* V;            /* [n_psr][n_gamma][ncp][ncp]: row j = eigenvector j of phi~_a^1/2 Z_a phi~_a^1/2 times
+                                 phi~_a^1/2; zero in rows and columns >= nc; 16-byte aligned                       */
+  const double* lam;          /* [n_psr][n_gamma][ncp]: eigenvalues (>= 0), zero past nc                           */
+  const double* a2;           /* [n_amp] A^2 = 10^(2 log10_A)                                                      */
+  const double* ldet;         /* [n_psr][n_gamma][n_amp]                                                           */
+} ptar_rn_model;
+
+/* lnL: [nreal][n_psr][n_gamma][n_amp]. */
+int ptar_rn_grid(const double* X, int32_t nreal, const ptar_rn_model* rm, double* lnL, void* stream);
 
 /* End-to-end job: GWB mix + synth + generate for realizations [real0, real0+nreal), then
  * (ptar_run_job_to_host) copy the residuals to pinned host memory, chunk by chunk, with the

@@ -20,6 +20,7 @@
 #include "ptar_os_aniso.cuh"
 #include "ptar_os_null.cuh"
 #include "ptar_os_pf.cuh"
+#include "ptar_rn.cuh"
 #include "ptar_rng.cuh"
 #include "ptar_timing.cuh"
 
@@ -642,8 +643,8 @@ int ptar_os_project_stage(const double* rows, int64_t ld, int32_t nreal, const p
     return fail(-1, "ptar_os_project: bad argument%s");
   if (!os->tiles || !os->tile0 || !os->n_tile || !os->C || os->n_tiles <= 0 || os->n_psr <= 0)
     return fail(-2, "ptar_os_project: model arrays missing%s");
-  if (!nc_ok(os->nc, os->ncp))
-    return fail(-2, "ptar_os_project: need 0 < nc <= 32 and ncp = nc rounded up to a multiple of 8%s");
+  if (!(os->nc > 0 && os->nc <= PTAR_RN_MAX_NC && os->ncp == ((os->nc + 7) & ~7)))   // the projection alone goes to 64
+    return fail(-2, "ptar_os_project: need 0 < nc <= 64 and ncp = nc rounded up to a multiple of 8%s");
   if ((ld & 3) || (reinterpret_cast<uintptr_t>(rows) & 31))
     return fail(-2, "ptar_os_project: rows must be 32-byte aligned with ld %% 4 == 0%s");
   if (os->n_tiles > 65535) return fail(-3, "ptar_os_project: more than 65535 tiles%s");
@@ -653,17 +654,22 @@ int ptar_os_project_stage(const double* rows, int64_t ld, int32_t nreal, const p
   if (stage != 2) {
     const dim3 grid(static_cast<unsigned>((nreal + ptar::OS_RB - 1) / ptar::OS_RB), static_cast<unsigned>(os->n_tiles));
     const int nt = os->ncp / 8;
-    static SmemOptIn optin[4];
+    static SmemOptIn optin[8];
     switch (nt) {
 #define PTAR_OS_LAUNCH(NT)                                                                                          \
   case NT:                                                                                                          \
-    if (int rc = opt_in_smem(ptar::os_project_kernel<NT>, optin[NT - 1], ptar::OS_SMEM, "ptar_os_project")) return rc; \
-    ptar::os_project_kernel<NT><<<grid, ptar::OS_THREADS, ptar::OS_SMEM, st>>>(rows, ld, nreal, *os, partial);      \
+    if (int rc = opt_in_smem(ptar::os_project_kernel<NT>, optin[NT - 1], ptar::os_project_smem(NT), "ptar_os_project")) \
+      return rc;                                                                                                    \
+    ptar::os_project_kernel<NT><<<grid, ptar::OS_THREADS, ptar::os_project_smem(NT), st>>>(rows, ld, nreal, *os, partial); \
     break;
       PTAR_OS_LAUNCH(1)
       PTAR_OS_LAUNCH(2)
       PTAR_OS_LAUNCH(3)
       PTAR_OS_LAUNCH(4)
+      PTAR_OS_LAUNCH(5)
+      PTAR_OS_LAUNCH(6)
+      PTAR_OS_LAUNCH(7)
+      PTAR_OS_LAUNCH(8)
 #undef PTAR_OS_LAUNCH
     }
     if (int rc = check_launch("ptar_os_project (tile GEMM)")) return rc;
@@ -961,6 +967,42 @@ int ptar_hd_grid(const double* X, int32_t nreal, const ptar_hd_model* hm, double
 #undef PTAR_HD_LAUNCH
   }
   return check_launch("ptar_hd_grid");
+}
+
+int ptar_rn_grid(const double* X, int32_t nreal, const ptar_rn_model* rm, double* lnL, void* stream) {
+  if (!X || !rm || !lnL || nreal <= 0) return fail(-1, "ptar_rn_grid: bad argument%s");
+  if (!rm->V || !rm->lam || !rm->a2 || !rm->ldet || rm->n_psr <= 0) return fail(-2, "ptar_rn_grid: model arrays missing%s");
+  if (!(rm->nc > 0 && rm->nc <= PTAR_RN_MAX_NC && rm->ncp == ((rm->nc + 7) & ~7)))
+    return fail(-2, "ptar_rn_grid: need 0 < nc <= 64 and ncp = nc rounded up to a multiple of 8%s");
+  if (!grid_ok(rm->n_amp, rm->n_gamma))
+    return fail(-2, "ptar_rn_grid: need 2 <= n_amp <= 256 and 1 <= n_gamma <= 256%s");
+  if ((reinterpret_cast<uintptr_t>(X) & 31) || (reinterpret_cast<uintptr_t>(rm->V) & 15))
+    return fail(-2, "ptar_rn_grid: X must be 32-byte aligned, V 16-byte aligned%s");
+  const int64_t nrb = (int64_t(nreal) + ptar::RN_RB - 1) / ptar::RN_RB;
+  const int64_t nz = int64_t(rm->n_psr) * ((rm->n_gamma + ptar::RN_GB - 1) / ptar::RN_GB);
+  if (nrb > 65535 || nz > 65535)
+    return fail(-3, "ptar_rn_grid: more than 65535 realization blocks or (pulsar, 16-gamma group) pairs%s");
+  const dim3 grid(static_cast<unsigned>((rm->n_amp + ptar::RN_AB - 1) / ptar::RN_AB), static_cast<unsigned>(nrb),
+                  static_cast<unsigned>(nz));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  static SmemOptIn optin[8];
+  switch (rm->ncp / 8) {
+#define PTAR_RN_LAUNCH(NT)                                                                                       \
+  case NT:                                                                                                       \
+    if (int rc = opt_in_smem(ptar::rn_grid_kernel<NT>, optin[NT - 1], ptar::RN_SMEM, "ptar_rn_grid")) return rc; \
+    ptar::rn_grid_kernel<NT><<<grid, ptar::RN_THREADS, ptar::RN_SMEM, st>>>(X, nreal, *rm, lnL);                 \
+    break;
+    PTAR_RN_LAUNCH(1)
+    PTAR_RN_LAUNCH(2)
+    PTAR_RN_LAUNCH(3)
+    PTAR_RN_LAUNCH(4)
+    PTAR_RN_LAUNCH(5)
+    PTAR_RN_LAUNCH(6)
+    PTAR_RN_LAUNCH(7)
+    PTAR_RN_LAUNCH(8)
+#undef PTAR_RN_LAUNCH
+  }
+  return check_launch("ptar_rn_grid");
 }
 
 int ptar_run_job_tm(const ptar_job* job, const ptar_timing_model* tm, double* scratch, int64_t scratch_len, int64_t real0,

@@ -11,7 +11,7 @@
 // os_project: grid = (realization blocks of 64, tiles), realization block fastest, so the CTAs that share a tile's
 // C rows run back to back and find them in L2 (C is read at 8 * ncp / 64 = 4 B per output at ncp = 32).  The
 // residual rows of a tile are staged 64 TOAs at a time by bulk-async copies (one copy per realization row) into a
-// 3-stage mbarrier ring; the products run on DMMA (mma.sync.m8n8k4.f64): M = 64 realizations, N = ncp <= 32 columns,
+// 3-stage mbarrier ring; the products run on DMMA (mma.sync.m8n8k4.f64): M = 64 realizations, N = ncp <= 64 columns,
 // K = TOAs.  Warp w owns m-tiles 4 (w & 1) .. +3 and the k-quarter w >> 1 of every 64-TOA chunk; the four
 // k-quarters are added in a fixed order at the end.  A partial therefore depends on the tile and the row's data
 // only -- not on which slot of which realization block the row landed in, nor on nreal, chunking or real0.  No
@@ -31,6 +31,13 @@ constexpr int OS_XP = OS_KC + 4;                 // smem row pitch (doubles): ro
 constexpr int OS_STAGES = 3;
 constexpr int OS_STAGE_DOUBLES = OS_RB * OS_XP;  // 34,816 B per stage
 constexpr size_t OS_SMEM = sizeof(double) * OS_STAGES * OS_STAGE_DOUBLES + 64;   // + barriers: 2 CTAs per SM
+// The ring also holds the k-quarter partials red[4][OS_RB][ncp] at the end; past ncp = 32 (NT > 4: the red-noise
+// likelihood's bases, up to ncp = 64) they outgrow it, so the barriers move behind them and one CTA runs per SM.
+__host__ __device__ constexpr int os_ring_doubles(int nt) {
+  return OS_STAGES * OS_STAGE_DOUBLES > 4 * OS_RB * 8 * nt ? OS_STAGES * OS_STAGE_DOUBLES : 4 * OS_RB * 8 * nt;
+}
+constexpr size_t os_project_smem(int nt) { return sizeof(double) * os_ring_doubles(nt) + 64; }   // == OS_SMEM for nt <= 4
+__host__ __device__ constexpr int os_ctas_per_sm(int nt) { return nt <= 4 ? 2 : 1; }
 constexpr int OS_PAIR_THREADS = 256;
 
 #define PTAR_OS_DMMA(c0, c1, a, b)                                                                      \
@@ -80,11 +87,12 @@ __device__ __forceinline__ void os_issue_chunk(double* stage, uint64_t* bar, con
 }
 
 template <int NT>   // n-tiles of 8 columns: ncp = 8 NT
-__global__ void __launch_bounds__(OS_THREADS, 2) os_project_kernel(const double* __restrict__ rows, int64_t ld, int nreal,
-                                                                   ptar_os_model os, double* __restrict__ partial) {
+__global__ void __launch_bounds__(OS_THREADS, os_ctas_per_sm(NT))
+    os_project_kernel(const double* __restrict__ rows, int64_t ld, int nreal, ptar_os_model os,
+                      double* __restrict__ partial) {
   extern __shared__ __align__(16) double os_smem[];
   constexpr int NCP = 8 * NT;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(os_smem + OS_STAGES * OS_STAGE_DOUBLES);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(os_smem + os_ring_doubles(NT));
   const ptar_tile tile = os.tiles[blockIdx.y];
   const int rb0 = blockIdx.x * OS_RB;
   const int nrow = min(OS_RB, nreal - rb0);
