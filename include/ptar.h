@@ -545,7 +545,8 @@ typedef struct {
   double ul;                  /* upper-limit quantile in (0, 1)                                                    */
 } ptar_curn_model;
 
-/* lnL: [nreal][n_gamma][n_amp]. */
+/* ptar_curn_grid reads every field; ptar_curn_reduce reads, and checks, only the grid: log10_A, wg, wx, prior, n_amp,
+ * n_gamma and ul.  lnL: [nreal][n_gamma][n_amp]. */
 int ptar_curn_grid(const double* X, int32_t nreal, const ptar_curn_model* cm, double* lnL, void* stream);
 /* lnL_max, ln_bayes, ul_amp: [nreal]; ml_gamma, ml_amp: [nreal] int64; post_amp: [nreal][n_amp];
  * post_gamma: [nreal][n_gamma]. */
@@ -592,7 +593,7 @@ int ptar_hd_grid(const double* X, int32_t nreal, const ptar_hd_model* hm, double
  *                 w_j = A_k^2 / (1 + A_k^2 lambda_j): two chained GEMMs on the fp64 tensor cores, no sum over pulsars.
  *                 X: [nreal][n_psr][ncp], 32-byte aligned.
  * The summaries of the nreal * n_psr maps [r][a] are ptar_curn_reduce's, called with nreal * n_psr and a
- * ptar_curn_model carrying the grid (log10_A, wg, wx, prior, ul, n_amp, n_gamma).  Outputs are bit-identical whatever
+ * ptar_curn_model carrying only the grid (log10_A, wg, wx, prior, ul, n_amp, n_gamma).  Outputs are bit-identical whatever
  * nreal, chunking or real0. */
 typedef struct {
   int32_t n_psr;              /* n_psr * ceil(n_gamma / 16) <= 65535                                               */

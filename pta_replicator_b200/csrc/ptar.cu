@@ -632,9 +632,9 @@ int ptar_timing_project(double* out, int64_t ld_out, int32_t nreal, const ptar_t
   return ptar_timing_project_stage(out, ld_out, nreal, tm, scratch, scratch_len, 0, stream);
 }
 
-// The basis width of the projection X [nreal][n_psr][ncp] (0 < nc <= 32, ncp = nc rounded up to a multiple of 8) and
-// the (log10 A, gamma) grid of the CURN and HD likelihoods (2 <= n_amp <= 256, 1 <= n_gamma <= 256).
-static inline bool nc_ok(int32_t nc, int32_t ncp) { return nc > 0 && nc <= PTAR_OS_MAX_NC && ncp == ((nc + 7) & ~7); }
+// The basis width of the projection X [nreal][n_psr][ncp] (0 < nc <= max, ncp = nc rounded up to a multiple of 8) and
+// the (log10 A, gamma) grid of the CURN, HD and red-noise likelihoods (2 <= n_amp <= 256, 1 <= n_gamma <= 256).
+static inline bool nc_ok(int32_t nc, int32_t ncp, int32_t max = PTAR_OS_MAX_NC) { return nc > 0 && nc <= max && ncp == ((nc + 7) & ~7); }
 static inline bool grid_ok(int32_t na, int32_t ng) { return na >= 2 && na <= PTAR_CURN_MAX_NA && ng >= 1 && ng <= PTAR_CURN_MAX_NG; }
 
 int ptar_os_project_stage(const double* rows, int64_t ld, int32_t nreal, const ptar_os_model* os, double* partial,
@@ -643,7 +643,7 @@ int ptar_os_project_stage(const double* rows, int64_t ld, int32_t nreal, const p
     return fail(-1, "ptar_os_project: bad argument%s");
   if (!os->tiles || !os->tile0 || !os->n_tile || !os->C || os->n_tiles <= 0 || os->n_psr <= 0)
     return fail(-2, "ptar_os_project: model arrays missing%s");
-  if (!(os->nc > 0 && os->nc <= PTAR_RN_MAX_NC && os->ncp == ((os->nc + 7) & ~7)))   // the projection alone goes to 64
+  if (!nc_ok(os->nc, os->ncp, PTAR_RN_MAX_NC))   // the projection alone goes to 64
     return fail(-2, "ptar_os_project: need 0 < nc <= 64 and ncp = nc rounded up to a multiple of 8%s");
   if ((ld & 3) || (reinterpret_cast<uintptr_t>(rows) & 31))
     return fail(-2, "ptar_os_project: rows must be 32-byte aligned with ld %% 4 == 0%s");
@@ -890,11 +890,8 @@ int ptar_fe_combine(const double* fmax, const int64_t* fargmax, int32_t nreal, c
   return check_launch("ptar_fe_combine");
 }
 
-static int curn_model_check(const ptar_curn_model* cm, const char* what) {
-  if (!cm->V || !cm->lam || !cm->a2 || !cm->ldet || !cm->log10_A || !cm->wg || !cm->wx || !cm->prior || cm->n_psr <= 0)
-    return fail(-2, "%s: model arrays missing", what);
-  if (!nc_ok(cm->nc, cm->ncp))
-    return fail(-2, "%s: need 0 < nc <= 32 and ncp = nc rounded up to a multiple of 8", what);
+static int curn_grid_check(const ptar_curn_model* cm, const char* what) {
+  if (!cm->log10_A || !cm->wg || !cm->wx || !cm->prior) return fail(-2, "%s: model arrays missing", what);
   if (!grid_ok(cm->n_amp, cm->n_gamma))
     return fail(-2, "%s: need 2 <= n_amp <= 256 and 1 <= n_gamma <= 256", what);
   if (!(cm->ul > 0.0 && cm->ul < 1.0)) return fail(-2, "%s: need 0 < ul < 1", what);
@@ -903,7 +900,9 @@ static int curn_model_check(const ptar_curn_model* cm, const char* what) {
 
 int ptar_curn_grid(const double* X, int32_t nreal, const ptar_curn_model* cm, double* lnL, void* stream) {
   if (!X || !cm || !lnL || nreal <= 0) return fail(-1, "ptar_curn_grid: bad argument%s");
-  if (int rc = curn_model_check(cm, "ptar_curn_grid")) return rc;
+  if (!cm->V || !cm->lam || !cm->a2 || !cm->ldet || cm->n_psr <= 0) return fail(-2, "ptar_curn_grid: model arrays missing%s");
+  if (!nc_ok(cm->nc, cm->ncp)) return fail(-2, "ptar_curn_grid: need 0 < nc <= 32 and ncp = nc rounded up to a multiple of 8%s");
+  if (int rc = curn_grid_check(cm, "ptar_curn_grid")) return rc;
   if ((reinterpret_cast<uintptr_t>(X) & 31) || (reinterpret_cast<uintptr_t>(cm->V) & 15))
     return fail(-2, "ptar_curn_grid: X must be 32-byte aligned, V 16-byte aligned%s");
   const int64_t nrb = (int64_t(nreal) + ptar::CURN_RB - 1) / ptar::CURN_RB;
@@ -932,7 +931,7 @@ int ptar_curn_reduce(const double* lnL, int32_t nreal, const ptar_curn_model* cm
                      void* stream) {
   if (!lnL || !cm || !lnL_max || !ml_gamma || !ml_amp || !ln_bayes || !post_amp || !post_gamma || !ul_amp || nreal <= 0)
     return fail(-1, "ptar_curn_reduce: bad argument%s");
-  if (int rc = curn_model_check(cm, "ptar_curn_reduce")) return rc;
+  if (int rc = curn_grid_check(cm, "ptar_curn_reduce")) return rc;
   ptar::curn_reduce_kernel<<<static_cast<unsigned>(nreal), ptar::CURN_RED_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(
       lnL, nreal, *cm, lnL_max, ml_gamma, ml_amp, ln_bayes, post_amp, post_gamma, ul_amp);
   return check_launch("ptar_curn_reduce");
@@ -972,7 +971,7 @@ int ptar_hd_grid(const double* X, int32_t nreal, const ptar_hd_model* hm, double
 int ptar_rn_grid(const double* X, int32_t nreal, const ptar_rn_model* rm, double* lnL, void* stream) {
   if (!X || !rm || !lnL || nreal <= 0) return fail(-1, "ptar_rn_grid: bad argument%s");
   if (!rm->V || !rm->lam || !rm->a2 || !rm->ldet || rm->n_psr <= 0) return fail(-2, "ptar_rn_grid: model arrays missing%s");
-  if (!(rm->nc > 0 && rm->nc <= PTAR_RN_MAX_NC && rm->ncp == ((rm->nc + 7) & ~7)))
+  if (!nc_ok(rm->nc, rm->ncp, PTAR_RN_MAX_NC))
     return fail(-2, "ptar_rn_grid: need 0 < nc <= 64 and ncp = nc rounded up to a multiple of 8%s");
   if (!grid_ok(rm->n_amp, rm->n_gamma))
     return fail(-2, "ptar_rn_grid: need 2 <= n_amp <= 256 and 1 <= n_gamma <= 256%s");

@@ -37,6 +37,63 @@ constexpr size_t CURN_SMEM = sizeof(double) * (CURN_STAGES * CURN_STAGE_DOUBLES 
                                                PTAR_OS_MAX_NC * CURN_WP) + 16;   // + barriers: 141,328 B
 constexpr int CURN_RED_THREADS = 256;                        // >= PTAR_CURN_MAX_NA and PTAR_CURN_MAX_NG
 
+// The per-pulsar body of curn_grid_kernel and rn_grid_kernel (ptar_rn.cuh): a CTA of CURN_THREADS threads over
+// CURN_RB realizations x CURN_AB amplitudes, warp w owning the realization rows 8w .. 8w + 7.
+
+// w_j(A) = A^2 / (1 + A^2 lambda_j) [ncp x 64] of the amplitudes k0 .. k0 + 63, the IEEE expression of the host oracle
+// (no contraction); 0 past n_amp
+template <int NCP>
+__device__ __forceinline__ void grid_w_tile(double* ws, const double* lam, const double* a2s, int k0, int NA, int tid) {
+  for (int e = tid; e < NCP * CURN_AB; e += CURN_THREADS) {
+    const int j = e / CURN_AB, n = e % CURN_AB;
+    const double a2 = k0 + n < NA ? __ldg(a2s + k0 + n) : 0.0;
+    ws[j * CURN_WP + n] = __ddiv_rn(a2, __dadd_rn(1.0, __dmul_rn(a2, __ldg(lam + j))));
+  }
+}
+
+// The warp's rows of Y = X_a V_a^T (M = 8, N = ncp, K = ncp) from X_a and V_a staged at pitch OS_XP, squared into its
+// own rows yw of Y^2 (pitch YP); the caller's __syncwarp publishes them
+template <int NT, int YP>
+__device__ __forceinline__ void grid_y2_rows(double* yw, const double* xs, const double* vs, int warp, int fr, int fk) {
+  constexpr int NCP = 8 * NT;
+  double y[NT][2];
+#pragma unroll
+  for (int t = 0; t < NT; ++t) y[t][0] = y[t][1] = 0.0;
+#pragma unroll
+  for (int kk = 0; kk < NCP; kk += 4) {
+    const double af = xs[(warp * 8 + fr) * OS_XP + kk + fk];
+#pragma unroll
+    for (int t = 0; t < NT; ++t) PTAR_OS_DMMA(y[t][0], y[t][1], af, vs[(t * 8 + fr) * OS_XP + kk + fk]);
+  }
+#pragma unroll
+  for (int t = 0; t < NT; ++t) {
+    yw[fr * YP + t * 8 + 2 * fk] = __dmul_rn(y[t][0], y[t][0]);
+    yw[fr * YP + t * 8 + 2 * fk + 1] = __dmul_rn(y[t][1], y[t][1]);
+  }
+}
+
+// Q += Y^2 W (M = 8, N = 64, K = ncp) on the warp's rows of Y^2
+template <int NCP, int YP>
+__device__ __forceinline__ void grid_q_add(double (&q)[8][2], const double* yw, const double* ws, int fr, int fk) {
+#pragma unroll
+  for (int kk = 0; kk < NCP; kk += 4) {
+    const double af = yw[fr * YP + kk + fk];
+#pragma unroll
+    for (int t = 0; t < 8; ++t) PTAR_OS_DMMA(q[t][0], q[t][1], af, ws[(kk + fk) * CURN_WP + t * 8 + fr]);
+  }
+}
+
+// out[k] = 1/2 (Q - ldet[k]) of the thread's row at its amplitudes k0 + 8t + 2 fk + c < n_amp
+__device__ __forceinline__ void grid_store(double* out, const double* ld, const double (&q)[8][2], int k0, int NA, int fk) {
+#pragma unroll
+  for (int t = 0; t < 8; ++t)
+#pragma unroll
+    for (int c = 0; c < 2; ++c) {
+      const int k = k0 + t * 8 + 2 * fk + c;
+      if (k < NA) out[k] = __dmul_rn(0.5, __dsub_rn(q[t][c], __ldg(ld + k)));
+    }
+}
+
 template <int NT>   // n-tiles of 8 basis columns: ncp = 8 NT
 __global__ void __launch_bounds__(CURN_THREADS, 1) curn_grid_kernel(const double* __restrict__ X, int nreal,
                                                                    ptar_curn_model cm, double* __restrict__ lnL) {
@@ -74,50 +131,18 @@ __global__ void __launch_bounds__(CURN_THREADS, 1) curn_grid_kernel(const double
     const int s = a % CURN_STAGES;
     const double* xs = curn_smem + s * CURN_STAGE_DOUBLES;
     const double* vs = xs + CURN_RB * OS_XP;
-    // w_j(A) = A^2 / (1 + A^2 lambda_j), the IEEE expression of the host oracle (no contraction); 0 past n_amp
-    const double* lam = cm.lam + (int64_t(a) * NG + g) * NCP;
-    for (int e = tid; e < NCP * CURN_AB; e += CURN_THREADS) {
-      const int j = e / CURN_AB, n = e % CURN_AB;
-      const double a2 = k0 + n < NA ? __ldg(cm.a2 + k0 + n) : 0.0;
-      ws[j * CURN_WP + n] = __ddiv_rn(a2, __dadd_rn(1.0, __dmul_rn(a2, __ldg(lam + j))));
-    }
+    grid_w_tile<NCP>(ws, cm.lam + (int64_t(a) * NG + g) * NCP, cm.a2, k0, NA, tid);
     os_mbar_wait(bars + s, (a / CURN_STAGES) & 1);
     __syncthreads();   // W complete
-    double y[NT][2];
-#pragma unroll
-    for (int t = 0; t < NT; ++t) y[t][0] = y[t][1] = 0.0;
-#pragma unroll
-    for (int kk = 0; kk < NCP; kk += 4) {
-      const double af = xs[(warp * 8 + fr) * OS_XP + kk + fk];
-#pragma unroll
-      for (int t = 0; t < NT; ++t) PTAR_OS_DMMA(y[t][0], y[t][1], af, vs[(t * 8 + fr) * OS_XP + kk + fk]);
-    }
-#pragma unroll
-    for (int t = 0; t < NT; ++t) {
-      yw[fr * CURN_YP + t * 8 + 2 * fk] = __dmul_rn(y[t][0], y[t][0]);
-      yw[fr * CURN_YP + t * 8 + 2 * fk + 1] = __dmul_rn(y[t][1], y[t][1]);
-    }
+    grid_y2_rows<NT, CURN_YP>(yw, xs, vs, warp, fr, fk);
     __syncwarp();
-#pragma unroll
-    for (int kk = 0; kk < NCP; kk += 4) {
-      const double af = yw[fr * CURN_YP + kk + fk];
-#pragma unroll
-      for (int t = 0; t < 8; ++t) PTAR_OS_DMMA(q[t][0], q[t][1], af, ws[(kk + fk) * CURN_WP + t * 8 + fr]);
-    }
+    grid_q_add<NCP, CURN_YP>(q, yw, ws, fr, fk);
     __syncthreads();   // stage s, W and Y^2 are free
     if (warp == 0 && a + CURN_STAGES < P) issue(a + CURN_STAGES);
   }
   const int r = warp * 8 + fr;
   if (r >= nrow) return;
-  double* out = lnL + (int64_t(rb0 + r) * NG + g) * NA;
-  const double* ld = cm.ldet + int64_t(g) * NA;
-#pragma unroll
-  for (int t = 0; t < 8; ++t)
-#pragma unroll
-    for (int c = 0; c < 2; ++c) {
-      const int k = k0 + t * 8 + 2 * fk + c;
-      if (k < NA) out[k] = __dmul_rn(0.5, __dsub_rn(q[t][c], __ldg(ld + k)));
-    }
+  grid_store(lnL + (int64_t(rb0 + r) * NG + g) * NA, cm.ldet + int64_t(g) * NA, q, k0, NA, fk);
 }
 
 // One CTA per realization, over its map lnL[g][k] (k = log10 A index).  Every sum runs in a fixed order: per-thread

@@ -23,19 +23,19 @@
 #include <stdint.h>
 
 #include "../../include/ptar.h"
+#include "ptar_curn.cuh"
 #include "ptar_os.cuh"
 
 namespace ptar {
 
-constexpr int RN_THREADS = 256;
-constexpr int RN_RB = 64;                                    // realizations per CTA (one m-tile of 8 per warp)
-constexpr int RN_AB = 64;                                    // amplitudes per CTA (8 n-tiles)
+constexpr int RN_THREADS = CURN_THREADS;                     // the CTA shape of the body shared with curn_grid_kernel
+constexpr int RN_RB = CURN_RB;                               // realizations per CTA (one m-tile of 8 per warp)
+constexpr int RN_AB = CURN_AB;                               // amplitudes per CTA (8 n-tiles)
 constexpr int RN_STAGES = 2;                                 // V_a(gamma) buffers
 constexpr int RN_GB = 16;                                    // gammas per CTA
 constexpr int RN_YP = PTAR_RN_MAX_NC + 4;                    // Y^2 pitch: rows 32 B apart -> conflict-free A gathers
-constexpr int RN_WP = RN_AB + 8;                             // W pitch: k rows 64 B apart -> conflict-free B gathers
 constexpr size_t RN_SMEM = sizeof(double) * (RN_RB * OS_XP + RN_STAGES * PTAR_RN_MAX_NC * OS_XP + RN_RB * RN_YP +
-                                             PTAR_RN_MAX_NC * RN_WP) + 32;   // + 3 barriers: 176,160 B
+                                             PTAR_RN_MAX_NC * CURN_WP) + 32;   // + 3 barriers: 176,160 B
 
 template <int NT>   // n-tiles of 8 basis columns: ncp = 8 NT
 __global__ void __launch_bounds__(RN_THREADS, 1) rn_grid_kernel(const double* __restrict__ X, int nreal, ptar_rn_model m,
@@ -46,7 +46,7 @@ __global__ void __launch_bounds__(RN_THREADS, 1) rn_grid_kernel(const double* __
   double* vring = xs + RN_RB * OS_XP;
   double* ys = vring + RN_STAGES * PTAR_RN_MAX_NC * OS_XP;
   double* ws = ys + RN_RB * RN_YP;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(ws + PTAR_RN_MAX_NC * RN_WP);   // [0, RN_STAGES) V stages, then X
+  uint64_t* bars = reinterpret_cast<uint64_t*>(ws + PTAR_RN_MAX_NC * CURN_WP);   // [0, RN_STAGES) V stages, then X
   const int P = m.n_psr, NA = m.n_amp, NG = m.n_gamma, ngg = (NG + RN_GB - 1) / RN_GB;
   const int k0 = blockIdx.x * RN_AB, rb0 = blockIdx.y * RN_RB, a = blockIdx.z / ngg;
   const int g0 = (blockIdx.z % ngg) * RN_GB, ng = min(RN_GB, NG - g0);
@@ -74,51 +74,18 @@ __global__ void __launch_bounds__(RN_THREADS, 1) rn_grid_kernel(const double* __
   for (int i = 0; i < ng; ++i) {
     const int g = g0 + i, s = i % RN_STAGES;
     const double* vs = vring + s * PTAR_RN_MAX_NC * OS_XP;
-    // w_j(A) = A^2 / (1 + A^2 lambda_j), the IEEE expression of the host oracle (no contraction); 0 past n_amp
-    const double* lam = m.lam + (int64_t(a) * NG + g) * NCP;
-    for (int e = tid; e < NCP * RN_AB; e += RN_THREADS) {
-      const int j = e / RN_AB, n = e % RN_AB;
-      const double a2 = k0 + n < NA ? __ldg(m.a2 + k0 + n) : 0.0;
-      ws[j * RN_WP + n] = __ddiv_rn(a2, __dadd_rn(1.0, __dmul_rn(a2, __ldg(lam + j))));
-    }
+    grid_w_tile<NCP>(ws, m.lam + (int64_t(a) * NG + g) * NCP, m.a2, k0, NA, tid);
     if (i == 0) os_mbar_wait(bars + RN_STAGES, 0);
     os_mbar_wait(bars + s, (i / RN_STAGES) & 1);
     __syncthreads();   // W complete
-    double y[NT][2];
-#pragma unroll
-    for (int t = 0; t < NT; ++t) y[t][0] = y[t][1] = 0.0;
-#pragma unroll
-    for (int kk = 0; kk < NCP; kk += 4) {
-      const double af = xs[(warp * 8 + fr) * OS_XP + kk + fk];
-#pragma unroll
-      for (int t = 0; t < NT; ++t) PTAR_OS_DMMA(y[t][0], y[t][1], af, vs[(t * 8 + fr) * OS_XP + kk + fk]);
-    }
-#pragma unroll
-    for (int t = 0; t < NT; ++t) {
-      yw[fr * RN_YP + t * 8 + 2 * fk] = __dmul_rn(y[t][0], y[t][0]);
-      yw[fr * RN_YP + t * 8 + 2 * fk + 1] = __dmul_rn(y[t][1], y[t][1]);
-    }
+    grid_y2_rows<NT, RN_YP>(yw, xs, vs, warp, fr, fk);
     __syncwarp();
     double q[8][2];
 #pragma unroll
     for (int t = 0; t < 8; ++t) q[t][0] = q[t][1] = 0.0;
-#pragma unroll
-    for (int kk = 0; kk < NCP; kk += 4) {
-      const double af = yw[fr * RN_YP + kk + fk];
-#pragma unroll
-      for (int t = 0; t < 8; ++t) PTAR_OS_DMMA(q[t][0], q[t][1], af, ws[(kk + fk) * RN_WP + t * 8 + fr]);
-    }
-    if (r < nrow) {
-      double* out = lnL + ((int64_t(rb0 + r) * P + a) * NG + g) * NA;
-      const double* ld = m.ldet + (int64_t(a) * NG + g) * NA;
-#pragma unroll
-      for (int t = 0; t < 8; ++t)
-#pragma unroll
-        for (int c = 0; c < 2; ++c) {
-          const int k = k0 + t * 8 + 2 * fk + c;
-          if (k < NA) out[k] = __dmul_rn(0.5, __dsub_rn(q[t][c], __ldg(ld + k)));
-        }
-    }
+    grid_q_add<NCP, RN_YP>(q, yw, ws, fr, fk);
+    if (r < nrow)
+      grid_store(lnL + ((int64_t(rb0 + r) * P + a) * NG + g) * NA, m.ldet + (int64_t(a) * NG + g) * NA, q, k0, NA, fk);
     __syncthreads();   // stage s, W and Y^2 are free
     if (warp == 0 && i + RN_STAGES < ng) issue(i + RN_STAGES);
   }

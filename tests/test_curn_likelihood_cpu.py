@@ -134,3 +134,29 @@ def test_missing_white_noise_raises_in_plan():
     b.set_curn_likelihood()
     with pytest.raises(ValueError, match="CURN likelihood needs white noise"):
         b.plan()
+
+
+def test_curn_model_checks_refuse_before_any_launch():
+    """``ptar_curn_reduce`` checks only the grid fields it reads, ``ptar_curn_grid`` those and the per-pulsar forms;
+    both refuse a bad model before anything reaches a device."""
+    import ctypes as C
+
+    from pta_replicator_b200 import _cabi
+    L = _cabi.lib()
+    buf = (C.c_double * 64)()
+    p = C.addressof(buf)                                  # never read: every call below stops at its checks
+
+    def model(**kw):
+        f = dict(n_psr=1, nc=2, ncp=8, n_gamma=3, n_amp=6, V=p, lam=p, a2=p, ldet=p, log10_A=p, wg=p, wx=p, prior=p, ul=0.95)
+        return _cabi.CurnModel(**{**f, **kw})
+
+    calls = dict(reduce=lambda m: L.ptar_curn_reduce(p, 4, C.byref(m), *([p] * 7), None),
+                 grid=lambda m: L.ptar_curn_grid(p, 4, C.byref(m), p, None))
+    for kw, msg, which in ((dict(log10_A=None), "model arrays missing", calls), (dict(wg=None), "model arrays missing", calls),
+                           (dict(wx=None), "model arrays missing", calls), (dict(prior=None), "model arrays missing", calls),
+                           (dict(n_amp=1), "2 <= n_amp", calls), (dict(ul=1.0), "0 < ul < 1", calls),
+                           (dict(V=None), "model arrays missing", ("grid",)), (dict(nc=0), "0 < nc <= 32", ("grid",))):
+        for name in which:
+            assert calls[name](model(**kw)) == -2, (name, kw)
+            err = L.ptar_last_error().decode()
+            assert msg in err and f"ptar_curn_{name}" in err, (name, kw, err)

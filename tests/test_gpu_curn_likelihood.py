@@ -176,6 +176,13 @@ def test_bit_identity_across_chunk_real0_maps_and_paths():
     rows = b.generate(R, seed=SEED)                    # no timing model: the pre-fit rows the statistic reduces
     _equal(a, b.curn_likelihood_of(rows, maps=True), KEYS + ("lnL",))
     _equal(a, b.curn_likelihood_of(rows), KEYS)
+    per_real = 8 * 9 * 70
+    for n_sub in (40, 128):                             # map scratch sub-blocks below and above one realization block
+        b.GRID_MAP_BYTES = n_sub * per_real
+        t = {}
+        _equal(a, b.curn_likelihood_of(rows, timers=t), KEYS)
+        assert sum(1 for e in t["events"] if e[0] == "curn_grid") == -(-R // n_sub)
+    del b.GRID_MAP_BYTES
     _check_summaries(a, np.linspace(-17, -12.5, 70), np.linspace(1, 6, 9))
 
 

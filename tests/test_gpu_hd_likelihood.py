@@ -164,6 +164,14 @@ def test_bit_identity_across_chunk_real0_maps_and_paths():
     rows = b.generate(R, seed=SEED)
     _equal(a, b.curn_likelihood_of(rows, maps=True), KEYS + HD_KEYS + ("lnL", "hd_lnL"))
     _equal(a, b.curn_likelihood_of(rows), KEYS + HD_KEYS)
+    per_real = 8 * len(gam) * len(x)
+    for n_sub in (40, 128):                             # map scratch sub-blocks below and above one realization block
+        b.GRID_MAP_BYTES = n_sub * per_real
+        t = {}
+        _equal(a, b.curn_likelihood_of(rows, timers=t), KEYS + HD_KEYS)
+        for name in ("curn_grid", "hd_grid"):
+            assert sum(1 for e in t["events"] if e[0] == name) == -(-R // n_sub), name
+    del b.GRID_MAP_BYTES
     _check_summaries(_hd_view(a), x, gam)
     _check_bayes(a)
 

@@ -167,11 +167,11 @@ def test_bit_identity_across_chunk_subblocks_real0_maps_and_paths():
     _equal(a, b.red_noise_likelihood_of(rows, maps=True), KEYS + ("lnL",))
     per_real = 8 * b.n_psr * len(gam) * len(x)
     for n_sub in (40, 128):                             # map scratch sub-blocks below and above one realization block
-        b.RN_MAP_BYTES = n_sub * per_real
+        b.GRID_MAP_BYTES = n_sub * per_real
         t = {}
         _equal(a, b.red_noise_likelihood_of(rows, timers=t), KEYS)
         assert sum(1 for e in t["events"] if e[0] == "rn_grid") == -(-R // n_sub)
-    del b.RN_MAP_BYTES
+    del b.GRID_MAP_BYTES
     _check_summaries(a, x, gam)
 
 

@@ -46,10 +46,8 @@ def curn_reduce(st, ul, maps):
     from pta_replicator_b200 import _cabi
     R, NG, NA = maps.shape
     dev = {k: _t(st[k]) for k in ("log10_A", "wg", "wx", "prior")}
-    dummy = _t(np.zeros(4))
-    m = _cabi.CurnModel(n_psr=1, nc=2, ncp=8, n_gamma=NG, n_amp=NA, V=dummy.data_ptr(), lam=dummy.data_ptr(),
-                        a2=dummy.data_ptr(), ldet=dummy.data_ptr(), log10_A=dev["log10_A"].data_ptr(),
-                        wg=dev["wg"].data_ptr(), wx=dev["wx"].data_ptr(), prior=dev["prior"].data_ptr(), ul=float(ul))
+    m = _cabi.CurnModel(n_gamma=NG, n_amp=NA, log10_A=dev["log10_A"].data_ptr(), wg=dev["wg"].data_ptr(),
+                        wx=dev["wx"].data_ptr(), prior=dev["prior"].data_ptr(), ul=float(ul))
     lnL = _t(maps)
     out = dict(lnL_max=_empty(R), ml_gamma_index=_empty(R, "int64"), ml_log10_A_index=_empty(R, "int64"),
                ln_bayes=_empty(R), post_log10_A=_empty((R, NA)), post_gamma=_empty((R, NG)), log10_A_ul=_empty(R))
