@@ -11,7 +11,8 @@
  *
  * Non-finite inputs.  The summary entry points take maps and statistics a caller may supply, so NaN and +-inf reach
  * them in normal use; they follow one rule.
- *   - Every (max, argmax) -- ptar_curn_reduce, ptar_fp_reduce, ptar_fe_sky, ptar_fe_combine, ptar_os_aniso -- ranks by
+ *   - Every (max, argmax) -- ptar_curn_reduce, ptar_fp_reduce, ptar_fe_sky, ptar_fe_combine, ptar_os_aniso,
+ *     ptar_bwm_sky, ptar_bwm_combine -- ranks by
  *     larger value, then lower index, with NaN above every number: the first NaN wins wherever it sits, otherwise the
  *     first maximum.
  *   - ptar_curn_reduce: -inf among finite entries is a zero likelihood and everything stays finite.  A NaN or +inf
@@ -55,6 +56,9 @@
  *                          ORF-correlated common-process likelihood on the CURN grid, reduced by ptar_curn_reduce
  *   ptar_rn_grid           no counterpart (a single-pulsar noise analysis per realization and pulsar): each pulsar's
  *                          intrinsic red-noise likelihood on an (A, gamma) grid, reduced by ptar_curn_reduce
+ *   ptar_bwm_sky /         no counterpart (a matched-filter search of add_gw_memory's ramp per realization): the
+ *   ptar_bwm_combine       coherent burst-with-memory statistic over epoch x sky and the pulsar-term statistic, reduced
+ *                          on the device
  */
 #ifndef PTAR_H
 #define PTAR_H
@@ -75,7 +79,8 @@ extern "C" {
                              ptar_fp_project, ptar_fp_reduce[_fap], PTAR_FP_MAX_FREQ), the CURN likelihood
                              (ptar_curn_model, ptar_curn_grid, ptar_curn_reduce, PTAR_CURN_MAX_NA / _NG) and the HD
                              likelihood (ptar_hd_model, ptar_hd_grid, PTAR_HD_MAX_N / _JB) and the single-pulsar
-                             red-noise likelihood (ptar_rn_model, ptar_rn_grid, PTAR_RN_MAX_NC) are new symbols only, so
+                             red-noise likelihood (ptar_rn_model, ptar_rn_grid, PTAR_RN_MAX_NC) and the burst-with-memory
+                             search (ptar_bwm_model, ptar_bwm_sky, ptar_bwm_combine, PTAR_BWM_MAX_EPOCH) are new symbols only, so
                              a caller detects them by looking the symbol up.  ptar_os_project accepts nc up to
                              PTAR_RN_MAX_NC since the red-noise likelihood; nothing changes for nc <= PTAR_OS_MAX_NC. */
 
@@ -448,7 +453,8 @@ int ptar_os_pf(const double* X, int32_t nreal, const ptar_os_model* os, const pt
  *                    Fp_max[r] = max_f Fp[r][f], Fp_argmax[r] = the first f attaining it (the first NaN above every
  *                    number).
  * Every sum runs in an order fixed by the TOA index and the pulsar only: outputs are bit-identical whatever nreal,
- * chunking, real0 or launch grid produced the rows. */
+ * chunking, real0 or launch grid produced the rows.  The columns are generic: any whitened basis laid out as Ct is
+ * projected the same way (ptar_bwm_sky reads the projection of the whitened memory ramps, column j = epoch j). */
 #define PTAR_FP_MAX_FREQ 256   /* search frequencies (the reduce kernel: one thread per frequency) */
 typedef struct {
   int32_t n_psr;
@@ -507,6 +513,49 @@ int ptar_fe_sky(const double* amps, int32_t nreal, const ptar_fe_model* fe, doub
 /* fe_max, argmax_f, argmax_sky: [nreal]. */
 int ptar_fe_combine(const double* fmax, const int64_t* fargmax, int32_t nreal, const ptar_fe_model* fe, double* fe_max,
                     int64_t* argmax_f, int64_t* argmax_sky, void* stream);
+
+/* Burst-with-memory search over epoch x sky (csrc/ptar_bwm.cuh), from the amplitudes X^ of ptar_fp_project run with a
+ * ptar_fp_model whose Ct holds the whitened ramps (n_freq = ceil(T / 2), column j = epoch j, zero for an unseen epoch).
+ * The host derives, once per recipe, for every pulsar a and burst epoch t0 the ramp u = (t - t0) [t >= t0], its Fisher
+ * information m_a(t0) = u^T P_a^-1 u (P_a the noise covariance with the timing model marginalised; 0 for an epoch the
+ * pulsar does not see), C~_a(t0) = P_a^-1 u / sqrt(m_a(t0)), the Earth-term antenna patterns e_a(s) = (F+, Fx) and, per
+ * (t0, s), the inverse Cholesky factor of M2(t0, s) = sum_a e_a e_a^T m_a(t0).  Per realization r:
+ *   ptar_bwm_sky      N2[(r, t)][(s, pol)] = sum_a sqrt(m_a(t)) X^[r][a][t] e_a(s)[pol] on the fp64 tensor cores (the sum
+ *                     in pulsar order) with the epilogue B[r][t][s] = 1/2 |L2^-1 N2|^2 in registers (2B ~ chi^2_2 under the
+ *                     noise model); t0max[r][t] = max_s B, t0argmax[r][t] = the first s attaining it.  maps != NULL also
+ *                     writes B [nreal][n_t0][n_sky]; otherwise no map is written.
+ *   ptar_bwm_combine  bwm_max[r] = max_t t0max[r][t], argmax_t0[r] = the first t attaining it, argmax_sky[r] = its
+ *                     t0argmax; fap[r] = exp(-bwm_max); at that cell b^ = M2^-1 N2 (N2 re-formed in pulsar order),
+ *                     strain[r] = |b^|, pol[r] = 1/2 atan2(b^_x, b^_+) mod pi.  Per (r, a) over the epochs a sees:
+ *                     psr_max[r][a] = max_t 1/2 X^[r][a][t]^2, psr_argmax_t0 the first t attaining it, psr_slope =
+ *                     X^ / sqrt(m_a(t)) there and psr_fap = erfc(sqrt(psr_max)); a pulsar that sees no epoch gets -inf,
+ *                     index -1 and NaN slope and fap.
+ * Outputs are bit-identical whatever nreal, chunking or real0 produced the amplitudes. */
+#define PTAR_BWM_MAX_EPOCH 512   /* burst epochs: 2 PTAR_FP_MAX_FREQ projection columns */
+typedef struct {
+  int32_t n_psr;              /* 1 .. PTAR_FE_MAX_PSR                                                              */
+  int32_t n_t0;               /* T: 1 .. PTAR_BWM_MAX_EPOCH                                                        */
+  int32_t n_sky;              /* S: 1 .. PTAR_FE_MAX_SKY                                                           */
+  int32_t n_sb;               /* sky blocks of 32: ceil(S / 32)                                                    */
+  int32_t kp;                 /* n_psr rounded up to a multiple of 16                                              */
+  int32_t reserved;
+  const double* sqm;          /* [ceil(T / 2)][n_psr][2]: sqrt(m_a(2 q + c)); zero for an unseen epoch and past T     */
+  const uint8_t* seen;        /* [n_psr][T]: 1 where pulsar a sees epoch t                                          */
+  const double* ant;          /* [n_sb][kp][64]: the layout of ptar_fe_model.ant                                   */
+  const double* antenna;      /* [n_psr][n_sky][2]: e_a(s) = (F+, Fx)                                              */
+  const double* linv;         /* [ceil(T / 2)][32 n_sb][6]: L2^-1 (00, 10, 11) of epoch 2 q, then of 2 q + 1; zero past
+                                 n_sky and T                                                                       */
+} ptar_bwm_model;
+
+/* amps: [nreal][n_psr][2 ceil(T / 2)] (ptar_fp_project); t0max: [nreal][n_t0]; t0argmax: [nreal][n_t0] int64. */
+int ptar_bwm_sky(const double* amps, int32_t nreal, const ptar_bwm_model* bw, double* t0max, int64_t* t0argmax,
+                 double* maps, void* stream);
+/* bwm_max, strain, pol, fap: [nreal]; argmax_t0, argmax_sky: [nreal] int64; psr_max, psr_slope, psr_fap: [nreal][n_psr];
+ * psr_argmax_t0: [nreal][n_psr] int64. */
+int ptar_bwm_combine(const double* amps, const double* t0max, const int64_t* t0argmax, int32_t nreal,
+                     const ptar_bwm_model* bw, double* bwm_max, int64_t* argmax_t0, int64_t* argmax_sky, double* strain,
+                     double* pol, double* fap, double* psr_max, int64_t* psr_argmax_t0, double* psr_slope,
+                     double* psr_fap, void* stream);
 
 /* Common uncorrelated red process (CURN) likelihood on an (A, gamma) grid (csrc/ptar_curn.cuh), from the X of
  * ptar_os_project run with a ptar_os_model that holds only the projection fields (tiles, tile0, n_tile, C, nc, ncp).

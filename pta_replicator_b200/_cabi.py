@@ -52,7 +52,7 @@ EXPORTS = ("ptar_version", "ptar_last_error", "ptar_cholesky_lower", "ptar_fouri
            "ptar_run_job_tm", "ptar_run_job_to_host_tm", "ptar_os_project", "ptar_os_project_stage", "ptar_os_pairs",
            "ptar_os_null", "ptar_os_null_stage", "ptar_os_aniso", "ptar_os_aniso_stage", "ptar_os_pf", "ptar_fp_project", "ptar_fp_reduce",
            "ptar_fp_reduce_fap", "ptar_fe_sky", "ptar_fe_combine", "ptar_curn_grid", "ptar_curn_reduce",
-           "ptar_hd_grid", "ptar_rn_grid")
+           "ptar_hd_grid", "ptar_rn_grid", "ptar_bwm_sky", "ptar_bwm_combine")
 OS_MAX_NC, OS_MAX_ORF, OS_MAX_PSR = 32, 4, 256     # optimal statistic: GW-basis columns, templates, pulsars (ptar.h)
 OS_MAX_NULL = 65536                                # null columns of ptar_os_null (PTAR_OS_MAX_NULL)
 OS_NULL_PHASE_SHIFT, OS_NULL_SKY_SCRAMBLE = 1, 2
@@ -64,6 +64,8 @@ FE_SB = 32                                         # sky points per stage of pta
 CURN_MAX_NA, CURN_MAX_NG = 256, 256                # CURN likelihood grid: log10 A and gamma points (ptar.h)
 HD_MAX_N, HD_JB = 4096, 32                         # HD likelihood: n_psr 2K eigen-rows, rows per block (ptar.h)
 RN_MAX_NC = 64                                     # red-noise likelihood: basis columns of ptar_rn_grid / ptar_os_project
+BWM_MAX_EPOCH = 512                                # burst-with-memory search: burst epochs (PTAR_BWM_MAX_EPOCH)
+BWM_LINV = 6                                       # packed L2^-1 doubles per (epoch pair, sky point) (csrc/ptar_bwm.cuh)
 
 
 class Tile(C.Structure):
@@ -135,6 +137,12 @@ class FpModel(C.Structure):
 class FeModel(C.Structure):
     _fields_ = [("n_psr", C.c_int32), ("n_freq", C.c_int32), ("n_sky", C.c_int32), ("n_sb", C.c_int32),
                 ("kp", C.c_int32), ("reserved", C.c_int32), ("Lf", C.c_void_p), ("ant", C.c_void_p), ("linv", C.c_void_p)]
+
+
+class BwmModel(C.Structure):
+    _fields_ = [("n_psr", C.c_int32), ("n_t0", C.c_int32), ("n_sky", C.c_int32), ("n_sb", C.c_int32),
+                ("kp", C.c_int32), ("reserved", C.c_int32), ("sqm", C.c_void_p), ("seen", C.c_void_p), ("ant", C.c_void_p),
+                ("antenna", C.c_void_p), ("linv", C.c_void_p)]
 
 
 class CurnModel(C.Structure):
@@ -213,6 +221,8 @@ def lib():
     L.ptar_fp_reduce_fap.argtypes = [vp, C.c_int32, vp, vp, vp, vp, vp, vp]
     L.ptar_fe_sky.argtypes = [vp, C.c_int32, vp, vp, vp, vp, vp]                         # fe: address of an FeModel
     L.ptar_fe_combine.argtypes = [vp, vp, C.c_int32, vp, vp, vp, vp, vp]
+    L.ptar_bwm_sky.argtypes = [vp, C.c_int32, vp, vp, vp, vp, vp]                        # bw: address of a BwmModel
+    L.ptar_bwm_combine.argtypes = [vp, vp, vp, C.c_int32, vp] + [vp] * 10 + [vp]
     L.ptar_curn_grid.argtypes = [vp, C.c_int32, vp, vp, vp]                           # cm: address of a CurnModel
     L.ptar_curn_reduce.argtypes = [vp, C.c_int32, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     L.ptar_hd_grid.argtypes = [vp, C.c_int32, vp, vp, vp]                             # hm: address of an HdModel

@@ -9,6 +9,7 @@
 #include <algorithm>
 
 #include "../../include/ptar.h"
+#include "ptar_bwm.cuh"
 #include "ptar_curn.cuh"
 #include "ptar_generate.cuh"
 #include "ptar_gwb.cuh"
@@ -888,6 +889,53 @@ int ptar_fe_combine(const double* fmax, const int64_t* fargmax, int32_t nreal, c
   ptar::fe_combine_kernel<<<blocks, ptar::FE_COMBINE_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(
       fmax, fargmax, nreal, fe->n_freq, fe_max, argmax_f, argmax_sky);
   return check_launch("ptar_fe_combine");
+}
+
+static int bwm_model_check(const ptar_bwm_model* bw, const char* what) {
+  if (!bw->sqm || !bw->seen || !bw->ant || !bw->antenna || !bw->linv) return fail(-2, "%s: model arrays missing", what);
+  if (bw->n_psr < 1 || bw->n_psr > PTAR_FE_MAX_PSR || bw->kp != ((bw->n_psr + 15) & ~15))
+    return fail(-2, "%s: need 1 <= n_psr <= 128 and kp = n_psr rounded up to a multiple of 16", what);
+  if (bw->n_t0 < 1 || bw->n_t0 > PTAR_BWM_MAX_EPOCH) return fail(-2, "%s: need 1 <= n_t0 <= 512", what);
+  if (bw->n_sky < 1 || bw->n_sky > PTAR_FE_MAX_SKY || bw->n_sb != (bw->n_sky + ptar::FE_SB - 1) / ptar::FE_SB)
+    return fail(-2, "%s: need 1 <= n_sky <= 12288 and n_sb = ceil(n_sky / 32)", what);
+  if ((reinterpret_cast<uintptr_t>(bw->sqm) & 15) || (reinterpret_cast<uintptr_t>(bw->ant) & 15) ||
+      (reinterpret_cast<uintptr_t>(bw->linv) & 15))
+    return fail(-2, "%s: sqm, ant and linv must be 16-byte aligned", what);
+  return 0;
+}
+
+int ptar_bwm_sky(const double* amps, int32_t nreal, const ptar_bwm_model* bw, double* t0max, int64_t* t0argmax,
+                 double* maps, void* stream) {
+  if (!amps || !bw || !t0max || !t0argmax || nreal <= 0) return fail(-1, "ptar_bwm_sky: bad argument%s");
+  if (int rc = bwm_model_check(bw, "ptar_bwm_sky")) return rc;
+  if (reinterpret_cast<uintptr_t>(amps) & 15) return fail(-2, "ptar_bwm_sky: amps must be 16-byte aligned%s");
+  static SmemOptIn optin;
+  if (int rc = opt_in_smem(ptar::bwm_sky_kernel, optin, ptar::sky_smem_bytes(PTAR_FE_MAX_PSR, ptar::BWM_LINV),
+                           "ptar_bwm_sky"))
+    return rc;
+  const dim3 grid(static_cast<unsigned>((nreal + ptar::FE_RB - 1) / ptar::FE_RB), static_cast<unsigned>((bw->n_t0 + 1) / 2));
+  ptar::bwm_sky_kernel<<<grid, ptar::FE_THREADS, ptar::sky_smem_bytes(bw->kp, ptar::BWM_LINV),
+                         static_cast<cudaStream_t>(stream)>>>(amps, nreal, *bw, t0max, t0argmax, maps);
+  return check_launch("ptar_bwm_sky");
+}
+
+int ptar_bwm_combine(const double* amps, const double* t0max, const int64_t* t0argmax, int32_t nreal,
+                     const ptar_bwm_model* bw, double* bwm_max, int64_t* argmax_t0, int64_t* argmax_sky, double* strain,
+                     double* pol, double* fap, double* psr_max, int64_t* psr_argmax_t0, double* psr_slope,
+                     double* psr_fap, void* stream) {
+  if (!amps || !t0max || !t0argmax || !bw || !bwm_max || !argmax_t0 || !argmax_sky || !strain || !pol || !fap ||
+      !psr_max || !psr_argmax_t0 || !psr_slope || !psr_fap || nreal <= 0)
+    return fail(-1, "ptar_bwm_combine: bad argument%s");
+  if (int rc = bwm_model_check(bw, "ptar_bwm_combine")) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int T = ptar::BWM_COMBINE_THREADS;
+  ptar::bwm_combine_kernel<<<static_cast<unsigned>((nreal + T - 1) / T), T, 0, st>>>(
+      amps, t0max, t0argmax, nreal, *bw, bwm_max, argmax_t0, argmax_sky, strain, pol, fap);
+  if (int rc = check_launch("ptar_bwm_combine")) return rc;
+  const int64_t n = int64_t(nreal) * bw->n_psr;
+  ptar::bwm_psr_kernel<<<static_cast<unsigned>((n + T - 1) / T), T, 0, st>>>(amps, nreal, *bw, psr_max, psr_argmax_t0,
+                                                                            psr_slope, psr_fap);
+  return check_launch("ptar_bwm_combine (pulsar term)");
 }
 
 static int curn_grid_check(const ptar_curn_model* cm, const char* what) {

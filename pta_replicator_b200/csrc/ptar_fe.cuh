@@ -21,6 +21,8 @@
 // (max, first argmax) per thread.  The 8 x kp x 64 GEMM product of a stage is never written (with `maps` only Fe is).
 // Per thread the sky order is increasing, and the (max, lowest index) combine of the threads that hold a realization is
 // exact and order-free, so every output depends on the realization's amplitudes only.  No atomics anywhere.
+// The staged mainloop -- ring, barriers, operand staging, fragment gathers and the DMMA loop -- is sky_mainloop, which
+// bwm_sky_kernel (csrc/ptar_bwm.cuh) shares: a kernel supplies only its operand former and its per-cell epilogue.
 #pragma once
 #include <cuda_runtime.h>
 #include <math.h>
@@ -38,41 +40,50 @@ constexpr int FE_BN = 2 * FE_SB;          // columns (s, pol) per stage
 constexpr int FE_LINV = 10;               // packed lower-triangular L4^-1
 constexpr int FE_COMBINE_THREADS = 256;
 
-__host__ __device__ constexpr int fe_stage_doubles(int kp) { return kp * FE_BN + FE_SB * FE_LINV; }
-// N tile + two stages + two mbarriers: 199 KB at kp = 128 (1 CTA per SM), 130 KB at kp = 80
-__host__ __device__ constexpr size_t fe_smem_bytes(int kp) {
-  return sizeof(double) * (size_t(2 * FE_RB) * (kp + 4) + 2 * size_t(fe_stage_doubles(kp))) + 64;
+// A stage of a sky kernel: the antenna block [kp][64] and LINV packed doubles per sky point of the block.
+__host__ __device__ constexpr int sky_stage_doubles(int kp, int linv) { return kp * FE_BN + FE_SB * linv; }
+// N tile + two stages + two mbarriers
+__host__ __device__ constexpr size_t sky_smem_bytes(int kp, int linv) {
+  return sizeof(double) * (size_t(2 * FE_RB) * (kp + 4) + 2 * size_t(sky_stage_doubles(kp, linv))) + 64;
 }
+__host__ __device__ constexpr int fe_stage_doubles(int kp) { return sky_stage_doubles(kp, FE_LINV); }
+// 199 KB at kp = 128 (1 CTA per SM), 130 KB at kp = 80
+__host__ __device__ constexpr size_t fe_smem_bytes(int kp) { return sky_smem_bytes(kp, FE_LINV); }
 static_assert(fe_smem_bytes(PTAR_FE_MAX_PSR) <= 227 * 1024, "the Fe tile must fit one SM's shared memory");
 static_assert(PTAR_FE_MAX_PSR % 16 == 0, "kp is a multiple of 16");
 
-// One thread fills stage `st` with sky block `sb`: the antenna block (all kp pulsars x 64 columns) and L4^-1 of (f, sb).
-__device__ __forceinline__ void fe_issue_stage(double* st, uint64_t* bar, const ptar_fe_model& fe, int f, int sb) {
-  const uint32_t ab = static_cast<uint32_t>(fe.kp) * FE_BN * 8u, lb = FE_SB * FE_LINV * 8u;
+// One thread fills stage `st` with sky block `sb`: the antenna block (all kp pulsars x 64 columns) and the LINV packed
+// doubles of each of its 32 sky points, row y (this CTA's frequency or epoch pair) of lv [y][32 n_sb][LINV].
+template <int LINV>
+__device__ __forceinline__ void sky_issue_stage(double* st, uint64_t* bar, const double* ant, const double* lv, int kp, int nsb,
+                                                int y, int sb) {
+  const uint32_t ab = static_cast<uint32_t>(kp) * FE_BN * 8u, lb = FE_SB * LINV * 8u;
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // earlier generic reads of this stage
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(os_smem_u32(bar)), "r"(ab + lb) : "memory");
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
                    os_smem_u32(st)),
-               "l"(fe.ant + int64_t(sb) * fe.kp * FE_BN), "r"(ab), "r"(os_smem_u32(bar))
+               "l"(ant + int64_t(sb) * kp * FE_BN), "r"(ab), "r"(os_smem_u32(bar))
                : "memory");
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                   os_smem_u32(st + fe.kp * FE_BN)),
-               "l"(fe.linv + (int64_t(f) * fe.n_sb + sb) * FE_SB * FE_LINV), "r"(lb), "r"(os_smem_u32(bar))
+                   os_smem_u32(st + kp * FE_BN)),
+               "l"(lv + (int64_t(y) * nsb + sb) * FE_SB * LINV), "r"(lb), "r"(os_smem_u32(bar))
                : "memory");
 }
 
-__global__ void __launch_bounds__(FE_THREADS, 1) fe_sky_kernel(const double* __restrict__ amps, int nreal, ptar_fe_model fe,
-                                                               double* __restrict__ fmax, int64_t* __restrict__ fargmax,
-                                                               double* __restrict__ maps) {
-  extern __shared__ __align__(16) double fe_smem[];
-  __shared__ double red_v[2][FE_RB];
-  __shared__ int red_i[2][FE_RB];
-  const int kp = fe.kp, ap = kp + 4, P = fe.n_psr, nsb = fe.n_sb;
-  const int sd = fe_stage_doubles(kp);
-  double* As = fe_smem;                                   // [c][FE_RB][ap]
-  double* ring = fe_smem + 2 * FE_RB * ap;                // 2 x [kp][64] antenna + [32][10] L4^-1
+// The staged mainloop of the sky kernels (fe_sky_kernel, bwm_sky_kernel).  The CTA's 64 x kp operand N is formed
+// once by form(m, a, n0, n1) (realization slot m, pulsar a; rows c = 0 and c = 1; both 0 on entry), then the sky is
+// walked 32 points per stage through the 2-stage bulk-async ring of antenna blocks `ant` [n_sb][kp][64] and packed
+// per-point factors, row y of `lv` [y][32 n_sb][LINV].  After each stage's DMMA loop every thread calls epi(sky, L, v0, v1, v2, v3)
+// for its four sky points in increasing order, with L the point's LINV factors and (v0, v1, v2, v3) = N2 of
+// (c = 0, +), (c = 1, +), (c = 0, x), (c = 1, x) for its realization slot row = 8 (warp & 3) + (lane >> 2).
+template <int LINV, class Form, class Epi>
+__device__ __forceinline__ void sky_mainloop(const double* ant, const double* lv, int kp, int nsb, int y, Form form, Epi epi) {
+  extern __shared__ __align__(16) double sky_smem[];
+  const int ap = kp + 4;
+  const int sd = sky_stage_doubles(kp, LINV);
+  double* As = sky_smem;                                  // [c][FE_RB][ap]
+  double* ring = sky_smem + 2 * FE_RB * ap;               // 2 x [kp][64] antenna + [32][LINV] factors
   uint64_t* bars = reinterpret_cast<uint64_t*>(ring + 2 * sd);
-  const int f = blockIdx.y, r0 = blockIdx.x * FE_RB, nrow = min(FE_RB, nreal - r0);
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   if (tid == 0) {
     for (int s = 0; s < 2; ++s) asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(os_smem_u32(bars + s)));
@@ -80,18 +91,11 @@ __global__ void __launch_bounds__(FE_THREADS, 1) fe_sky_kernel(const double* __r
   }
   __syncthreads();
   if (tid == 0)
-    for (int s = 0; s < 2 && s < nsb; ++s) fe_issue_stage(ring + s * sd, bars + s, fe, f, s);
-  // N = L_a(f) X^ of this CTA's realizations at frequency f; zero past nreal and n_psr
-  const int64_t nc = 2 * int64_t(fe.n_freq);
+    for (int s = 0; s < 2 && s < nsb; ++s) sky_issue_stage<LINV>(ring + s * sd, bars + s, ant, lv, kp, nsb, y, s);
   for (int e = tid; e < FE_RB * kp; e += FE_THREADS) {
     const int m = e / kp, a = e - m * kp;
     double n0 = 0.0, n1 = 0.0;
-    if (m < nrow && a < P) {
-      const double2 x = *reinterpret_cast<const double2*>(amps + (int64_t(r0 + m) * P + a) * nc + 2 * f);
-      const double* l = fe.Lf + (int64_t(f) * P + a) * 3;
-      n0 = __dmul_rn(l[0], x.x);
-      n1 = __fma_rn(l[1], x.x, __dmul_rn(l[2], x.y));
-    }
+    form(m, a, n0, n1);
     As[m * ap + a] = n0;
     As[(FE_RB + m) * ap + a] = n1;
   }
@@ -101,9 +105,6 @@ __global__ void __launch_bounds__(FE_THREADS, 1) fe_sky_kernel(const double* __r
   const int row = wm * 8 + fr;                            // realization slot of this thread's accumulator rows
   const double* a0 = As + row * ap + fk;                  // c = 0
   const double* a1 = As + (FE_RB + row) * ap + fk;        // c = 1
-  double* mrow = (maps && row < nrow) ? maps + (int64_t(r0 + row) * fe.n_freq + f) * fe.n_sky : nullptr;
-  double best = -INFINITY;
-  int bidx = 0x7fffffff;
   for (int sb = 0; sb < nsb; ++sb) {
     const int s = sb & 1;
     double* bs = ring + s * sd;
@@ -129,25 +130,49 @@ __global__ void __launch_bounds__(FE_THREADS, 1) fe_sky_kernel(const double* __r
 #pragma unroll
     for (int t = 0; t < 4; ++t) {
       const int sl = wn * 16 + t * 4 + fk;               // columns 2 sl (+), 2 sl + 1 (x) of the stage
-      const int sky = sb * FE_SB + sl;
-      const double* L = li + sl * FE_LINV;
-      const double v0 = acc[0][t][0], v1 = acc[1][t][0], v2 = acc[0][t][1], v3 = acc[1][t][1];
-      const double y0 = __dmul_rn(L[0], v0);
-      const double y1 = __fma_rn(L[1], v0, __dmul_rn(L[2], v1));
-      const double y2 = __fma_rn(L[3], v0, __fma_rn(L[4], v1, __dmul_rn(L[5], v2)));
-      const double y3 = __fma_rn(L[6], v0, __fma_rn(L[7], v1, __fma_rn(L[8], v2, __dmul_rn(L[9], v3))));
-      const double v = __dmul_rn(0.5, __fma_rn(y3, y3, __fma_rn(y2, y2, __fma_rn(y1, y1, __dmul_rn(y0, y0)))));
-      if (sky < fe.n_sky) {
-        if (fe_better(v, sky, best, bidx)) {
-          best = v;
-          bidx = sky;
-        }
-        if (mrow) mrow[sky] = v;
-      }
+      epi(sb * FE_SB + sl, li + sl * LINV, acc[0][t][0], acc[1][t][0], acc[0][t][1], acc[1][t][1]);
     }
     __syncthreads();   // every warp is done with stage s
-    if (tid == 0 && sb + 2 < nsb) fe_issue_stage(bs, bars + s, fe, f, sb + 2);
+    if (tid == 0 && sb + 2 < nsb) sky_issue_stage<LINV>(bs, bars + s, ant, lv, kp, nsb, y, sb + 2);
   }
+}
+
+__global__ void __launch_bounds__(FE_THREADS, 1) fe_sky_kernel(const double* __restrict__ amps, int nreal, ptar_fe_model fe,
+                                                               double* __restrict__ fmax, int64_t* __restrict__ fargmax,
+                                                               double* __restrict__ maps) {
+  __shared__ double red_v[2][FE_RB];
+  __shared__ int red_i[2][FE_RB];
+  const int P = fe.n_psr;
+  const int f = blockIdx.y, r0 = blockIdx.x * FE_RB, nrow = min(FE_RB, nreal - r0);
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int wn = warp >> 2, fk = lane & 3, row = (warp & 3) * 8 + (lane >> 2);
+  const int64_t nc = 2 * int64_t(fe.n_freq);
+  double best = -INFINITY;
+  int bidx = 0x7fffffff;
+  // N = L_a(f) X^ of this CTA's realizations at frequency f; zero past nreal and n_psr
+  auto form = [&](int m, int a, double& n0, double& n1) {
+    if (m < nrow && a < P) {
+      const double2 x = *reinterpret_cast<const double2*>(amps + (int64_t(r0 + m) * P + a) * nc + 2 * f);
+      const double* l = fe.Lf + (int64_t(f) * P + a) * 3;
+      n0 = __dmul_rn(l[0], x.x);
+      n1 = __fma_rn(l[1], x.x, __dmul_rn(l[2], x.y));
+    }
+  };
+  auto epi = [&](int sky, const double* L, double v0, double v1, double v2, double v3) {
+    const double y0 = __dmul_rn(L[0], v0);
+    const double y1 = __fma_rn(L[1], v0, __dmul_rn(L[2], v1));
+    const double y2 = __fma_rn(L[3], v0, __fma_rn(L[4], v1, __dmul_rn(L[5], v2)));
+    const double y3 = __fma_rn(L[6], v0, __fma_rn(L[7], v1, __fma_rn(L[8], v2, __dmul_rn(L[9], v3))));
+    const double v = __dmul_rn(0.5, __fma_rn(y3, y3, __fma_rn(y2, y2, __fma_rn(y1, y1, __dmul_rn(y0, y0)))));
+    if (sky < fe.n_sky) {
+      if (fe_better(v, sky, best, bidx)) {
+        best = v;
+        bidx = sky;
+      }
+      if (maps && row < nrow) maps[(int64_t(r0 + row) * fe.n_freq + f) * fe.n_sky + sky] = v;
+    }
+  };
+  sky_mainloop<FE_LINV>(fe.ant, fe.linv, fe.kp, fe.n_sb, f, form, epi);
   // (max, first argmax) over the threads of a realization: the quad (fk), then the two column halves (wn)
 #pragma unroll
   for (int o = 1; o < 4; o <<= 1) {
