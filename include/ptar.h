@@ -56,6 +56,9 @@
  *                          ORF-correlated common-process likelihood on the CURN grid, reduced by ptar_curn_reduce
  *   ptar_rn_grid           no counterpart (a single-pulsar noise analysis per realization and pulsar): each pulsar's
  *                          intrinsic red-noise likelihood on an (A, gamma) grid, reduced by ptar_curn_reduce
+ *   ptar_fs_grid           no counterpart (an MCMC over enterprise's free_spectrum model per realization): the
+ *                          factorised free-spectrum likelihood, one log10 rho grid per GW frequency bin, uncorrelated or
+ *                          ORF-correlated, reduced by ptar_curn_reduce
  *   ptar_bwm_sky /         no counterpart (a matched-filter search of add_gw_memory's ramp per realization): the
  *   ptar_bwm_combine       coherent burst-with-memory statistic over epoch x sky and the pulsar-term statistic, reduced
  *                          on the device
@@ -80,7 +83,8 @@ extern "C" {
                              (ptar_curn_model, ptar_curn_grid, ptar_curn_reduce, PTAR_CURN_MAX_NA / _NG) and the HD
                              likelihood (ptar_hd_model, ptar_hd_grid, PTAR_HD_MAX_N / _JB) and the single-pulsar
                              red-noise likelihood (ptar_rn_model, ptar_rn_grid, PTAR_RN_MAX_NC) and the burst-with-memory
-                             search (ptar_bwm_model, ptar_bwm_sky, ptar_bwm_combine, PTAR_BWM_MAX_EPOCH) are new symbols only, so
+                             search (ptar_bwm_model, ptar_bwm_sky, ptar_bwm_combine, PTAR_BWM_MAX_EPOCH) and the
+                             free-spectrum likelihood (ptar_fs_model, ptar_fs_grid, PTAR_FS_MAX_PSR / _BIN / _JB) are new symbols only, so
                              a caller detects them by looking the symbol up.  ptar_os_project accepts nc up to
                              PTAR_RN_MAX_NC since the red-noise likelihood; nothing changes for nc <= PTAR_OS_MAX_NC. */
 
@@ -660,6 +664,39 @@ typedef struct {
 
 /* lnL: [nreal][n_psr][n_gamma][n_amp]. */
 int ptar_rn_grid(const double* X, int32_t nreal, const ptar_rn_model* rm, double* lnL, void* stream);
+
+/* Factorised free-spectrum likelihood on a log10 rho grid (csrc/ptar_fs.cuh), one 1-D grid per GW frequency bin k, from
+ * the X of ptar_os_project on the 2K columns of the bins (column pair k of C is P_a,k^{-1} F_k, P_a,k the noise model of
+ * bin k).  The model of bin k is a common process in bin k alone, phi_k = rho^2 per Fourier coefficient, uncorrelated
+ * (Gamma = I) or with an ORF Gamma = B B^T.  The host derives, once per recipe, for every bin the eigendecomposition
+ * G^T Z[k] G = U diag(lambda) U^T of size n = 2 n_psr (Z[k] = blockdiag_a F_k^T P_a,k^{-1} F_k, G = B (x) I_2),
+ * V_k = U^T G^T and ldet[k][i] = sum_j log1p(rho_i^2 lambda_j).  Per realization r:
+ *   ptar_fs_grid  lnL[r][k][i] = 1/2 sum_j w_j y_j^2 - 1/2 ldet[k][i],  y = V_k X_k[r] with X_k[r][2a + c] =
+ *                 X[r][a][2k + c] (the bin-k columns of every pulsar, gathered), w_j = rho_i^2 / (1 + rho_i^2 lambda_j):
+ *                 two chained GEMMs on the fp64 tensor cores, j and the gathered axis in index order.
+ *                 X: [nreal][n_psr][ncp], 32-byte aligned.
+ * The summaries of the nreal * n_bin maps [r][k] are ptar_curn_reduce's, called with nreal * n_bin and a ptar_curn_model
+ * carrying only the grid (log10_A = log10 rho, wg = {1}, wx, prior, ul, n_amp, n_gamma = 1).  Outputs are bit-identical
+ * whatever nreal, chunking or real0. */
+#define PTAR_FS_MAX_PSR 256     /* pulsars: n = 2 n_psr eigen-rows per bin                     */
+#define PTAR_FS_MAX_BIN 32      /* frequency bins (2K <= PTAR_RN_MAX_NC projection columns)    */
+#define PTAR_FS_JB      32      /* eigen-rows per block: np = 2 n_psr rounded up to a multiple of 32 */
+typedef struct {
+  int32_t n_psr;              /* 1 .. PTAR_FS_MAX_PSR                                                              */
+  int32_t ncp;                /* 2 n_bin rounded up to a multiple of 8 (as the ptar_os_model of the projection)    */
+  int32_t n_bin;              /* K, 1 .. PTAR_FS_MAX_BIN                                                           */
+  int32_t n_amp;              /* 2 .. PTAR_CURN_MAX_NA log10 rho points                                            */
+  int32_t n2p;                /* 2 n_psr rounded up to a multiple of 8: the row pitch of V                          */
+  int32_t np;                 /* 2 n_psr rounded up to a multiple of PTAR_FS_JB                                    */
+  const double* V;            /* [n_bin][np][n2p]: row j = eigenvector j of G^T Z[k] G times G^T on the gathered axis
+                                 (2a + c); zero in rows >= 2 n_psr and columns >= 2 n_psr; 16-byte aligned        */
+  const double* lam;          /* [n_bin][np]: eigenvalues (>= 0), zero past 2 n_psr                                */
+  const double* a2;           /* [n_amp] rho^2 = 10^(2 log10 rho)                                                  */
+  const double* ldet;         /* [n_bin][n_amp]                                                                    */
+} ptar_fs_model;
+
+/* lnL: [nreal][n_bin][n_amp]. */
+int ptar_fs_grid(const double* X, int32_t nreal, const ptar_fs_model* fm, double* lnL, void* stream);
 
 /* End-to-end job: GWB mix + synth + generate for realizations [real0, real0+nreal), then
  * (ptar_run_job_to_host) copy the residuals to pinned host memory, chunk by chunk, with the

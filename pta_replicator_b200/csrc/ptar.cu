@@ -17,6 +17,7 @@
 #include "ptar_hd.cuh"
 #include "ptar_fe.cuh"
 #include "ptar_fp.cuh"
+#include "ptar_fs.cuh"
 #include "ptar_os.cuh"
 #include "ptar_os_aniso.cuh"
 #include "ptar_os_null.cuh"
@@ -1153,3 +1154,24 @@ int ptar_run_job_to_host(const ptar_job* job, int64_t real0, int64_t nreal, int3
 }
 
 }  // extern "C"
+
+int ptar_fs_grid(const double* X, int32_t nreal, const ptar_fs_model* fm, double* lnL, void* stream) {
+  if (!X || !fm || !lnL || nreal <= 0) return fail(-1, "ptar_fs_grid: bad argument%s");
+  if (!fm->V || !fm->lam || !fm->a2 || !fm->ldet) return fail(-2, "ptar_fs_grid: model arrays missing%s");
+  if (fm->n_psr < 1 || fm->n_psr > PTAR_FS_MAX_PSR || fm->n_bin < 1 || fm->n_bin > PTAR_FS_MAX_BIN ||
+      !nc_ok(2 * fm->n_bin, fm->ncp, PTAR_RN_MAX_NC))
+    return fail(-2, "ptar_fs_grid: need 1 <= n_psr <= 256, 1 <= n_bin <= 32 and ncp = 2 n_bin rounded up to a multiple of 8%s");
+  if (fm->n2p != ((2 * fm->n_psr + 7) & ~7) || fm->np != (2 * fm->n_psr + PTAR_FS_JB - 1) / PTAR_FS_JB * PTAR_FS_JB)
+    return fail(-2, "ptar_fs_grid: need n2p = 2 n_psr rounded up to a multiple of 8 and np to a multiple of 32%s");
+  if (!grid_ok(fm->n_amp, 1)) return fail(-2, "ptar_fs_grid: need 2 <= n_amp <= 256%s");
+  if ((reinterpret_cast<uintptr_t>(X) & 31) || (reinterpret_cast<uintptr_t>(fm->V) & 15))
+    return fail(-2, "ptar_fs_grid: X must be 32-byte aligned, V 16-byte aligned%s");
+  const int64_t nrb = (int64_t(nreal) + ptar::FS_RB - 1) / ptar::FS_RB;
+  if (nrb > 65535) return fail(-3, "ptar_fs_grid: more than 65535 realization blocks%s");
+  const dim3 grid(static_cast<unsigned>((fm->n_amp + ptar::FS_AB - 1) / ptar::FS_AB), static_cast<unsigned>(nrb),
+                  static_cast<unsigned>(fm->n_bin));
+  static SmemOptIn optin;
+  if (int rc = opt_in_smem(ptar::fs_grid_kernel, optin, ptar::FS_SMEM, "ptar_fs_grid")) return rc;
+  ptar::fs_grid_kernel<<<grid, ptar::FS_THREADS, ptar::FS_SMEM, static_cast<cudaStream_t>(stream)>>>(X, nreal, *fm, lnL);
+  return check_launch("ptar_fs_grid");
+}
