@@ -350,6 +350,21 @@ int launch_timing(double* out, int64_t ld, int32_t nreal, const ptar_timing_mode
   return 0;
 }
 
+// The checks of the sky grid that the Fe and BWM models share: every model array present (``arrays``), n_psr and kp,
+// n_sky and n_sb, and the arrays the sky kernels stage 16-byte aligned: ant, linv and BWM's ``sqm`` (nullptr for Fe).
+// The caller checks the model's frequency or epoch count.
+template <class Model>
+int sky_model_check(const Model* m, bool arrays, const double* sqm, const char* what) {
+  if (!arrays || !m->ant || !m->linv) return fail(-2, "%s: model arrays missing", what);
+  if (m->n_psr < 1 || m->n_psr > PTAR_FE_MAX_PSR || m->kp != ((m->n_psr + 15) & ~15))
+    return fail(-2, "%s: need 1 <= n_psr <= 128 and kp = n_psr rounded up to a multiple of 16", what);
+  if (m->n_sky < 1 || m->n_sky > PTAR_FE_MAX_SKY || m->n_sb != (m->n_sky + ptar::FE_SB - 1) / ptar::FE_SB)
+    return fail(-2, "%s: need 1 <= n_sky <= 12288 and n_sb = ceil(n_sky / 32)", what);
+  if ((reinterpret_cast<uintptr_t>(sqm) | reinterpret_cast<uintptr_t>(m->ant) | reinterpret_cast<uintptr_t>(m->linv)) & 15)
+    return fail(-2, sqm ? "%s: sqm, ant and linv must be 16-byte aligned" : "%s: ant and linv must be 16-byte aligned", what);
+  return 0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -856,22 +871,11 @@ int ptar_fp_reduce(const double* amps, int32_t nreal, const ptar_fp_model* fp, d
   return ptar_fp_reduce_fap(amps, nreal, fp, Fp, Fp_max, Fp_argmax, nullptr, stream);
 }
 
-static int fe_model_check(const ptar_fe_model* fe, const char* what) {
-  if (!fe->Lf || !fe->ant || !fe->linv) return fail(-2, "%s: model arrays missing", what);
-  if (fe->n_psr < 1 || fe->n_psr > PTAR_FE_MAX_PSR || fe->kp != ((fe->n_psr + 15) & ~15))
-    return fail(-2, "%s: need 1 <= n_psr <= 128 and kp = n_psr rounded up to a multiple of 16", what);
-  if (fe->n_freq < 1 || fe->n_freq > PTAR_FP_MAX_FREQ) return fail(-2, "%s: need 1 <= n_freq <= 256", what);
-  if (fe->n_sky < 1 || fe->n_sky > PTAR_FE_MAX_SKY || fe->n_sb != (fe->n_sky + ptar::FE_SB - 1) / ptar::FE_SB)
-    return fail(-2, "%s: need 1 <= n_sky <= 12288 and n_sb = ceil(n_sky / 32)", what);
-  if ((reinterpret_cast<uintptr_t>(fe->ant) & 15) || (reinterpret_cast<uintptr_t>(fe->linv) & 15))
-    return fail(-2, "%s: ant and linv must be 16-byte aligned", what);
-  return 0;
-}
-
 int ptar_fe_sky(const double* amps, int32_t nreal, const ptar_fe_model* fe, double* fmax, int64_t* fargmax, double* maps,
                 void* stream) {
   if (!amps || !fe || !fmax || !fargmax || nreal <= 0) return fail(-1, "ptar_fe_sky: bad argument%s");
-  if (int rc = fe_model_check(fe, "ptar_fe_sky")) return rc;
+  if (int rc = sky_model_check(fe, fe->Lf, nullptr, "ptar_fe_sky")) return rc;
+  if (fe->n_freq < 1 || fe->n_freq > PTAR_FP_MAX_FREQ) return fail(-2, "ptar_fe_sky: need 1 <= n_freq <= 256%s");
   if (reinterpret_cast<uintptr_t>(amps) & 15) return fail(-2, "ptar_fe_sky: amps must be 16-byte aligned%s");
   static SmemOptIn optin;
   if (int rc = opt_in_smem(ptar::fe_sky_kernel, optin, ptar::fe_smem_bytes(PTAR_FE_MAX_PSR), "ptar_fe_sky")) return rc;
@@ -885,30 +889,19 @@ int ptar_fe_combine(const double* fmax, const int64_t* fargmax, int32_t nreal, c
                     int64_t* argmax_f, int64_t* argmax_sky, void* stream) {
   if (!fmax || !fargmax || !fe || !fe_max || !argmax_f || !argmax_sky || nreal <= 0)
     return fail(-1, "ptar_fe_combine: bad argument%s");
-  if (int rc = fe_model_check(fe, "ptar_fe_combine")) return rc;
+  if (int rc = sky_model_check(fe, fe->Lf, nullptr, "ptar_fe_combine")) return rc;
+  if (fe->n_freq < 1 || fe->n_freq > PTAR_FP_MAX_FREQ) return fail(-2, "ptar_fe_combine: need 1 <= n_freq <= 256%s");
   const unsigned blocks = static_cast<unsigned>((nreal + ptar::FE_COMBINE_THREADS - 1) / ptar::FE_COMBINE_THREADS);
   ptar::fe_combine_kernel<<<blocks, ptar::FE_COMBINE_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(
       fmax, fargmax, nreal, fe->n_freq, fe_max, argmax_f, argmax_sky);
   return check_launch("ptar_fe_combine");
 }
 
-static int bwm_model_check(const ptar_bwm_model* bw, const char* what) {
-  if (!bw->sqm || !bw->seen || !bw->ant || !bw->antenna || !bw->linv) return fail(-2, "%s: model arrays missing", what);
-  if (bw->n_psr < 1 || bw->n_psr > PTAR_FE_MAX_PSR || bw->kp != ((bw->n_psr + 15) & ~15))
-    return fail(-2, "%s: need 1 <= n_psr <= 128 and kp = n_psr rounded up to a multiple of 16", what);
-  if (bw->n_t0 < 1 || bw->n_t0 > PTAR_BWM_MAX_EPOCH) return fail(-2, "%s: need 1 <= n_t0 <= 512", what);
-  if (bw->n_sky < 1 || bw->n_sky > PTAR_FE_MAX_SKY || bw->n_sb != (bw->n_sky + ptar::FE_SB - 1) / ptar::FE_SB)
-    return fail(-2, "%s: need 1 <= n_sky <= 12288 and n_sb = ceil(n_sky / 32)", what);
-  if ((reinterpret_cast<uintptr_t>(bw->sqm) & 15) || (reinterpret_cast<uintptr_t>(bw->ant) & 15) ||
-      (reinterpret_cast<uintptr_t>(bw->linv) & 15))
-    return fail(-2, "%s: sqm, ant and linv must be 16-byte aligned", what);
-  return 0;
-}
-
 int ptar_bwm_sky(const double* amps, int32_t nreal, const ptar_bwm_model* bw, double* t0max, int64_t* t0argmax,
                  double* maps, void* stream) {
   if (!amps || !bw || !t0max || !t0argmax || nreal <= 0) return fail(-1, "ptar_bwm_sky: bad argument%s");
-  if (int rc = bwm_model_check(bw, "ptar_bwm_sky")) return rc;
+  if (int rc = sky_model_check(bw, bw->sqm && bw->seen && bw->antenna, bw->sqm, "ptar_bwm_sky")) return rc;
+  if (bw->n_t0 < 1 || bw->n_t0 > PTAR_BWM_MAX_EPOCH) return fail(-2, "ptar_bwm_sky: need 1 <= n_t0 <= 512%s");
   if (reinterpret_cast<uintptr_t>(amps) & 15) return fail(-2, "ptar_bwm_sky: amps must be 16-byte aligned%s");
   static SmemOptIn optin;
   if (int rc = opt_in_smem(ptar::bwm_sky_kernel, optin, ptar::sky_smem_bytes(PTAR_FE_MAX_PSR, ptar::BWM_LINV),
@@ -927,7 +920,8 @@ int ptar_bwm_combine(const double* amps, const double* t0max, const int64_t* t0a
   if (!amps || !t0max || !t0argmax || !bw || !bwm_max || !argmax_t0 || !argmax_sky || !strain || !pol || !fap ||
       !psr_max || !psr_argmax_t0 || !psr_slope || !psr_fap || nreal <= 0)
     return fail(-1, "ptar_bwm_combine: bad argument%s");
-  if (int rc = bwm_model_check(bw, "ptar_bwm_combine")) return rc;
+  if (int rc = sky_model_check(bw, bw->sqm && bw->seen && bw->antenna, bw->sqm, "ptar_bwm_combine")) return rc;
+  if (bw->n_t0 < 1 || bw->n_t0 > PTAR_BWM_MAX_EPOCH) return fail(-2, "ptar_bwm_combine: need 1 <= n_t0 <= 512%s");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int T = ptar::BWM_COMBINE_THREADS;
   ptar::bwm_combine_kernel<<<static_cast<unsigned>((nreal + T - 1) / T), T, 0, st>>>(
@@ -1153,8 +1147,6 @@ int ptar_run_job_to_host(const ptar_job* job, int64_t real0, int64_t nreal, int3
   return ptar_run_job_to_host_tm(job, nullptr, nullptr, 0, real0, nreal, chunk, out_host, dev_buf0, dev_buf1, stream0, stream1);
 }
 
-}  // extern "C"
-
 int ptar_fs_grid(const double* X, int32_t nreal, const ptar_fs_model* fm, double* lnL, void* stream) {
   if (!X || !fm || !lnL || nreal <= 0) return fail(-1, "ptar_fs_grid: bad argument%s");
   if (!fm->V || !fm->lam || !fm->a2 || !fm->ldet) return fail(-2, "ptar_fs_grid: model arrays missing%s");
@@ -1175,3 +1167,5 @@ int ptar_fs_grid(const double* X, int32_t nreal, const ptar_fs_model* fm, double
   ptar::fs_grid_kernel<<<grid, ptar::FS_THREADS, ptar::FS_SMEM, static_cast<cudaStream_t>(stream)>>>(X, nreal, *fm, lnL);
   return check_launch("ptar_fs_grid");
 }
+
+}  // extern "C"

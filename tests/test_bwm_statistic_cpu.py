@@ -199,3 +199,44 @@ def test_registration_leaves_other_statistics_unchanged():
             if isinstance(v, np.ndarray):
                 assert np.array_equal(v, both[key][k]), (key, k)
     assert both["bwm"]["n_t0"] == 6 and both["bwm"]["setup_s"] == b.bwm_setup_s
+
+
+def test_sky_model_checks_refuse_before_any_launch():
+    """``ptar_fe_sky`` / ``ptar_fe_combine`` and ``ptar_bwm_sky`` / ``ptar_bwm_combine`` share one check of the sky grid
+    (the model arrays, n_psr and kp, n_sky and n_sb, the 16-byte alignment of the staged arrays), and each checks its
+    frequency or epoch count; every call below refuses its model before anything reaches a device."""
+    import ctypes as C
+
+    from pta_replicator_b200 import _cabi
+    L = _cabi.lib()
+    buf = (C.c_double * 64)()
+    p = (C.addressof(buf) + 15) & ~15                     # 16-byte aligned, never read: every call stops at its checks
+    sky = dict(n_psr=3, kp=16, n_sky=40, n_sb=2, ant=p, linv=p)
+
+    def fe(**kw):
+        return _cabi.FeModel(**{**sky, "n_freq": 4, "Lf": p, **kw})
+
+    def bw(**kw):
+        return _cabi.BwmModel(**{**sky, "n_t0": 5, "sqm": p, "seen": p, "antenna": p, **kw})
+
+    shared = [(dict(ant=None), "model arrays missing"), (dict(linv=None), "model arrays missing"),
+              (dict(n_psr=0), "1 <= n_psr <= 128"), (dict(n_psr=129, kp=144), "1 <= n_psr <= 128"),
+              (dict(kp=32), "kp = n_psr rounded up"), (dict(n_sky=0, n_sb=0), "1 <= n_sky <= 12288"),
+              (dict(n_sb=1), "n_sb = ceil(n_sky / 32)"), (dict(n_sky=12289, n_sb=385), "1 <= n_sky <= 12288")]
+    fe_own = [(dict(Lf=None), "model arrays missing"), (dict(n_freq=0), "1 <= n_freq <= 256"),
+              (dict(n_freq=257), "1 <= n_freq <= 256"), (dict(ant=p + 8), ": ant and linv must be 16-byte aligned"),
+              (dict(linv=p + 8), ": ant and linv must be 16-byte aligned")]
+    bw_own = [(dict(sqm=None), "model arrays missing"), (dict(seen=None), "model arrays missing"),
+              (dict(antenna=None), "model arrays missing"), (dict(n_t0=0), "1 <= n_t0 <= 512"),
+              (dict(n_t0=513), "1 <= n_t0 <= 512"), (dict(sqm=p + 8), ": sqm, ant and linv must be 16-byte aligned"),
+              (dict(ant=p + 8), ": sqm, ant and linv must be 16-byte aligned"),
+              (dict(linv=p + 8), ": sqm, ant and linv must be 16-byte aligned")]
+    calls = {"ptar_fe_sky": (fe, fe_own, lambda m: L.ptar_fe_sky(p, 4, C.byref(m), p, p, None, None)),
+             "ptar_fe_combine": (fe, fe_own, lambda m: L.ptar_fe_combine(p, p, 4, C.byref(m), p, p, p, None)),
+             "ptar_bwm_sky": (bw, bw_own, lambda m: L.ptar_bwm_sky(p, 4, C.byref(m), p, p, None, None)),
+             "ptar_bwm_combine": (bw, bw_own, lambda m: L.ptar_bwm_combine(p, p, p, 4, C.byref(m), *([p] * 10), None))}
+    for name, (model, own, call) in calls.items():
+        for kw, msg in shared + own:
+            assert call(model(**kw)) == -2, (name, kw)
+            err = L.ptar_last_error().decode()
+            assert err.startswith(name + ": ") and msg in err, (name, kw, err)

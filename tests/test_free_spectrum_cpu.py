@@ -106,6 +106,8 @@ def test_identity_orf_reproduces_uncorrelated_model():
 
 def test_registration_leaves_other_statistics_unchanged():
     b = _batch(_small(), tm=True)
+    for key in ("os", "os_null", "os_aniso", "os_pf", "fp", "fe", "curn", "hd", "rn", "bwm", "fs"):
+        assert getattr(b, f"{key}_setup_s") is None, key               # a fresh batch has spent no time on any statics
     b.set_optimal_statistic()
     b.set_fp_statistic(n_freqs=5)
     b.set_curn_likelihood(log10_A=np.linspace(-15.5, -13, 4), gamma=[2.0, 4.0])

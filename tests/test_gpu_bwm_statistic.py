@@ -11,6 +11,7 @@ from tests import bwm_oracle as BO
 from tests import os_oracle as OO
 from tests import reduction_reference as RR
 from tests.test_bwm_statistic_cpu import bwm_of_layout, unpack_layout
+from tests.test_gpu_fe_statistic import _check_maxima
 from tests.test_gpu_fp_statistic import SEED, _models, _ng15
 from tests.test_gpu_reduction_edges import _rows      # noise, zero, timing-model-like and sinusoid rows, cycling
 
@@ -19,6 +20,7 @@ pytestmark = pytest.mark.gpu
 T = 100
 KEYS = ("bwm_max", "bwm_argmax_t0", "bwm_argmax_sky", "bwm_t0max", "bwm_t0argmax", "bwm_strain", "bwm_pol", "bwm_fap",
         "psr_max", "psr_argmax_t0", "psr_slope", "psr_fap")
+MAXIMA = ("bwm", "bwm_t0max", "bwm_t0argmax", "bwm_max", "bwm_argmax_t0", "bwm_argmax_sky")
 
 
 def _batch(psrs, noise, gwb=True, tm=True, **bwm):
@@ -38,20 +40,6 @@ def _layout(b):
     d = b.compile()["bwm"]
     return dict(sqm=d["sqm"].cpu().numpy(), ant=d["ant"].cpu().numpy(), linv=d["linv"].cpu().numpy(), n_t0=d["n_t0"],
                 n_sky=d["n_sky"])
-
-
-def _check_maxima(res, S):
-    """Every maximum and argmax equals the map's exactly (first index on ties, epoch-major)."""
-    import torch
-    B = res["bwm"]
-    assert torch.equal(res["bwm_t0max"], B.max(dim=2).values)
-    bm = B.cpu().numpy()
-    assert np.array_equal(res["bwm_t0argmax"].cpu().numpy(), np.argmax(bm, axis=2))
-    assert torch.equal(res["bwm_max"], res["bwm_t0max"].max(dim=1).values)
-    flat = np.argmax(bm.reshape(bm.shape[0], -1), axis=1)
-    assert np.array_equal(res["bwm_argmax_t0"].cpu().numpy(), flat // S)
-    assert np.array_equal(res["bwm_argmax_sky"].cpu().numpy(), flat % S)
-    assert torch.equal(res["bwm_fap"], torch.exp(-res["bwm_max"]))
 
 
 def _check_pulsar_term(res, seen):
@@ -93,7 +81,8 @@ def test_device_matches_numpy_ng15_full():
           f"{float(res['bwm_max'].min()):.1f} .. {float(res['bwm_max'].max()):.1f}; seen {int(res['seen'].sum())}/"
           f"{res['seen'].numel()}; host statics {res['setup_s']:.2f} s")
     assert err <= 1e-10
-    _check_maxima(res, S)
+    _check_maxima(res, S, MAXIMA)
+    assert torch.equal(res["bwm_fap"], torch.exp(-res["bwm_max"]))
     _check_pulsar_term(res, res["seen"].cpu().numpy())
     assert np.all(B <= 0.5 * np.sum(X * X, axis=1)[:, :, None] * (1 + 1e-12))
     assert torch.all((res["bwm_pol"] >= 0) & (res["bwm_pol"] < np.pi)) and torch.all(res["bwm_strain"] >= 0)
@@ -118,7 +107,8 @@ def test_bit_identity_across_chunks_real0_outputs_and_paths():
     for k in KEYS:
         assert torch.equal(a[k], bare[k]), k
     assert "bwm" not in bare and "amps" not in bare
-    _check_maxima(a, int(a["sky"].shape[0]))
+    _check_maxima(a, int(a["sky"].shape[0]), MAXIMA)
+    assert torch.equal(a["bwm_fap"], torch.exp(-a["bwm_max"]))
     # without a timing model the generated rows are the rows the statistic reduces
     b2 = _batch(psrs, noise, tm=False, n_epochs=T, nside=8)
     e = b2.bwm_statistic(R, seed=SEED, pulsars=True, maps=True)
@@ -200,7 +190,8 @@ def test_bwm_edges_against_extended_precision(P, T_, S, R):
     ratio = float(np.max(np.abs(dev[sub] - ref.astype(float)) / bound))
     print(f"\n[bwm edges] P={P} T={T_} S={S} R={R}: worst |dB| / bound {ratio:.3f}")
     assert ratio <= 1
-    _check_maxima(res, S)
+    _check_maxima(res, S, MAXIMA)
+    assert torch.equal(res["bwm_fap"], torch.exp(-res["bwm_max"]))
     _check_pulsar_term(res, res["seen"].cpu().numpy())
     st = b.compile()["bwm"]
     G = 4096

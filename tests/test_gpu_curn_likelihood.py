@@ -9,7 +9,7 @@ import pytest
 from tests import curn_oracle as CO
 from tests import reduction_reference as RR
 from tests import timing_oracle as TO
-from tests.test_gpu_reduction_edges import _poison, _rows, _t
+from tests.test_gpu_reduction_edges import _equal, _np, _poison, _rows, _t
 
 pytestmark = pytest.mark.gpu
 
@@ -17,10 +17,6 @@ SEED = 20250922
 X_GRID = np.linspace(-15.5, -13.0, 6)
 G_GRID = np.array([2.0, 13.0 / 3.0, 6.5])
 KEYS = ("lnL_max", "ml_gamma_index", "ml_log10_A_index", "ln_bayes", "post_log10_A", "post_gamma", "log10_A_ul")
-
-
-def _np(res):
-    return {k: v.cpu().numpy() for k, v in res.items() if hasattr(v, "cpu")}
 
 
 def _check_summaries(res, x, gam, kind="log-uniform", ul=0.95):
@@ -34,12 +30,6 @@ def _check_summaries(res, x, gam, kind="log-uniform", ul=0.95):
     np.testing.assert_allclose(r["post_log10_A"], ref["post_log10_A"], rtol=1e-11, atol=1e-14)
     np.testing.assert_allclose(r["post_gamma"], ref["post_gamma"], rtol=1e-11, atol=1e-14)
     np.testing.assert_allclose(r["log10_A_ul"], ref["log10_A_ul"], rtol=0, atol=1e-10)
-
-
-def _equal(a, c, keys=KEYS):
-    import torch
-    for k in keys:
-        assert torch.equal(a[k], c[k]), k
 
 
 def _xref(b, rows):

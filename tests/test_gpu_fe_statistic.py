@@ -18,6 +18,7 @@ pytestmark = pytest.mark.gpu
 NF = 100
 FE_KEYS = ("Fe_fmax", "Fe_fargmax", "Fe_max", "Fe_argmax_f", "Fe_argmax_sky", "Fe")
 FP_KEYS = ("Fp", "Fp_max", "Fp_argmax", "fap", "amps")
+FE_MAXIMA = ("Fe", "Fe_fmax", "Fe_fargmax", "Fe_max", "Fe_argmax_f", "Fe_argmax_sky")
 
 
 def _layout(b):
@@ -26,18 +27,20 @@ def _layout(b):
     return {k: d[k].cpu().numpy() for k in ("Lf", "ant", "linv")}, d["n_sky"]
 
 
-def _check_maxima(res, S):
-    """Fe_fmax / Fe_max and their argmaxes equal the maxima of the returned map exactly (first index on ties)."""
+def _check_maxima(res, S, names=FE_MAXIMA):
+    """The maxima of a sky statistic equal those of its returned map exactly (first index on ties).  ``names``: the map
+    [R, rows, S] (rows: frequencies or epochs), the per-row maximum over the sky and its argmax, the overall maximum and
+    its row and sky indices."""
     import torch
-    Fe = res["Fe"]
-    assert torch.equal(res["Fe_fmax"], Fe.max(dim=2).values)
-    fe = Fe.cpu().numpy()
-    assert np.array_equal(res["Fe_fargmax"].cpu().numpy(), np.argmax(fe, axis=2))
-    assert torch.equal(res["Fe_max"], res["Fe_fmax"].max(dim=1).values)
-    flat = np.argmax(fe.reshape(fe.shape[0], -1), axis=1)                   # frequency-major: lower f, then lower s
-    assert np.array_equal(res["Fe_argmax_f"].cpu().numpy(), flat // S)
-    assert np.array_equal(res["Fe_argmax_sky"].cpu().numpy(), flat % S)
-    assert int(res["Fe_fargmax"].max()) < S and int(res["Fe_argmax_sky"].max()) < S
+    m, row_max, row_arg, top, top_row, top_sky = names
+    assert torch.equal(res[row_max], res[m].max(dim=2).values)
+    mp = res[m].cpu().numpy()
+    assert np.array_equal(res[row_arg].cpu().numpy(), np.argmax(mp, axis=2))
+    assert torch.equal(res[top], res[row_max].max(dim=1).values)
+    flat = np.argmax(mp.reshape(mp.shape[0], -1), axis=1)                   # row-major: lower row, then lower s
+    assert np.array_equal(res[top_row].cpu().numpy(), flat // S)
+    assert np.array_equal(res[top_sky].cpu().numpy(), flat % S)
+    assert int(res[row_arg].max()) < S and int(res[top_sky].max()) < S
 
 
 def test_device_matches_numpy_ng15_full():

@@ -13,16 +13,12 @@ from tests import fs_oracle as FO
 from tests import reduction_reference as RR
 from tests.test_gpu_curn_likelihood import _ng15, _q_moments_check, _small_tm
 from tests.test_gpu_hd_likelihood import _ng15_epoch
-from tests.test_gpu_reduction_edges import _poison, _rows, _t
+from tests.test_gpu_reduction_edges import _equal, _np, _poison, _rows, _t
 
 pytestmark = pytest.mark.gpu
 
 SEED = 20251017
 KEYS = ("lnL_max", "ml_log10_rho_index", "ln_bayes", "post_log10_rho", "log10_rho_ul")
-
-
-def _np(res):
-    return {k: v.cpu().numpy() for k, v in res.items() if hasattr(v, "cpu")}
 
 
 def _check_summaries(res, x, prefix=""):
@@ -36,12 +32,6 @@ def _check_summaries(res, x, prefix=""):
     np.testing.assert_allclose(r[prefix + "post_log10_rho"].reshape(R * K, NR), ref["post_log10_A"], rtol=1e-11, atol=1e-14)
     np.testing.assert_allclose(r[prefix + "log10_rho_ul"].ravel(), ref["log10_A_ul"], rtol=0, atol=1e-10)
     assert not any(k.endswith(("ml_gamma_index", "post_gamma")) for k in res)
-
-
-def _equal(a, c, keys):
-    import torch
-    for k in keys:
-        assert torch.equal(a[k], c[k]), k
 
 
 def _xref(b, rows, prefix=""):

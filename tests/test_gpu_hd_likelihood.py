@@ -11,8 +11,8 @@ from tests import curn_oracle as CO
 from tests import hd_oracle as HO
 from tests import os_oracle as OO
 from tests import reduction_reference as RR
-from tests.test_gpu_curn_likelihood import KEYS, _check_summaries, _equal, _ng15, _np, _q_moments_check, _small_tm
-from tests.test_gpu_reduction_edges import _poison, _rows, _t
+from tests.test_gpu_curn_likelihood import KEYS, _check_summaries, _ng15, _q_moments_check, _small_tm
+from tests.test_gpu_reduction_edges import _equal, _np, _poison, _rows, _t
 
 pytestmark = pytest.mark.gpu
 

@@ -11,8 +11,8 @@ from scipy.special import ndtri
 
 from tests import reduction_reference as RR
 from tests import rn_oracle as RO
-from tests.test_gpu_curn_likelihood import G_GRID, KEYS, SEED, X_GRID, _equal, _ng15, _np, _small_tm
-from tests.test_gpu_reduction_edges import _poison, _rows, _t
+from tests.test_gpu_curn_likelihood import G_GRID, KEYS, SEED, X_GRID, _ng15, _small_tm
+from tests.test_gpu_reduction_edges import _equal, _np, _poison, _rows, _t
 
 pytestmark = pytest.mark.gpu
 

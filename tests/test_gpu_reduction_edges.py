@@ -58,6 +58,10 @@ def _t(b, a):
     return torch.from_numpy(np.ascontiguousarray(a)).to(b.device)
 
 
+def _np(res):
+    return {k: v.cpu().numpy() for k, v in res.items() if hasattr(v, "cpu")}
+
+
 def _equal(a, c, keys):
     import torch
     for k in keys:
