@@ -62,6 +62,9 @@
  *   ptar_bwm_sky /         no counterpart (a matched-filter search of add_gw_memory's ramp per realization): the
  *   ptar_bwm_combine       coherent burst-with-memory statistic over epoch x sky and the pulsar-term statistic, reduced
  *                          on the device
+ *   ptar_burst_ninv /      no counterpart (a wavelet search for add_burst / add_noise_transient per realization): the
+ *   ptar_burst_project /   coherent sine-Gaussian statistic over a t0 x f0 x Q bank x sky (with ptar_fe_sky) and the
+ *   ptar_burst_reduce      per-pulsar transient statistic, reduced on the device
  */
 #ifndef PTAR_H
 #define PTAR_H
@@ -84,7 +87,9 @@ extern "C" {
                              likelihood (ptar_hd_model, ptar_hd_grid, PTAR_HD_MAX_N / _JB) and the single-pulsar
                              red-noise likelihood (ptar_rn_model, ptar_rn_grid, PTAR_RN_MAX_NC) and the burst-with-memory
                              search (ptar_bwm_model, ptar_bwm_sky, ptar_bwm_combine, PTAR_BWM_MAX_EPOCH) and the
-                             free-spectrum likelihood (ptar_fs_model, ptar_fs_grid, PTAR_FS_MAX_PSR / _BIN / _JB) are new symbols only, so
+                             free-spectrum likelihood (ptar_fs_model, ptar_fs_grid, PTAR_FS_MAX_PSR / _BIN / _JB) and the sine-Gaussian
+                             burst search (ptar_burst_model, ptar_burst_ninv, ptar_burst_project, ptar_burst_reduce,
+                             PTAR_BURST_MAX_TEMPLATE / _GROUP / _TB) are new symbols only, so
                              a caller detects them by looking the symbol up.  ptar_os_project accepts nc up to
                              PTAR_RN_MAX_NC since the red-noise likelihood; nothing changes for nc <= PTAR_OS_MAX_NC. */
 
@@ -560,6 +565,71 @@ int ptar_bwm_combine(const double* amps, const double* t0max, const int64_t* t0a
                      const ptar_bwm_model* bw, double* bwm_max, int64_t* argmax_t0, int64_t* argmax_sky, double* strain,
                      double* pol, double* fap, double* psr_max, int64_t* psr_argmax_t0, double* psr_slope,
                      double* psr_fap, void* stream);
+
+/* Sine-Gaussian burst search over a t0 x f0 x Q template bank and the sky (csrc/ptar_burst.cuh).  Template j = (t0, f0,
+ * Q), tau = Q / (2 pi f0), W_j(t) = exp(-(t - t0)^2 / tau^2) (cos, sin)(2 pi f0 (t - t0)) on the TOAs of its static window
+ * [lo, hi) (the range spanning |t - t0| <= 6 tau; zero outside), t = MJD 86400.  The host derives, once per recipe, with
+ * P_a^-1 = N^-1 - N^-1 T S^-1 T^T N^-1 (N = white + ECORR, T = timing model, red noise and common basis, S = L_S L_S^T):
+ * the z columns N^-1 T L_S^-T (a ptar_fp_model: ptar_fp_project gives z_a = L_S^-1 T^T N^-1 r_a), H_a(j) =
+ * L_S^-1 T^T N^-1 W_j, M_a(j) = W_j^T P_a^-1 W_j = L L^T and the sky statics of ptar_fe_sky.  Per realization r:
+ *   ptar_burst_ninv     y = N^-1 r on the packed axis (1/d per TOA, one Sherman-Morrison term per ECORR run, runs summed
+ *                       in TOA order); only the TOAs of the runs are written.
+ *   ptar_burst_project  for the templates of group g (bank indices 256 g .. 256 g + Jg - 1, Jg <= PTAR_BURST_GROUP):
+ *                       amps[r][a][2 jl + c] = (L^-1 (W_j^T y_a - H_a(j)^T z_a))[c], 0 for an unseen (a, j): the layout of
+ *                       ptar_fp_project with n_freq = Jg, so ptar_fe_sky (Lf = l11, l21, l22 of M_a(j)) runs on it unchanged.
+ *                       W_j is generated per TOA chunk on the device; the GEMM runs on the fp64 tensor cores and walks only
+ *                       the union of a 16-template block's windows.  y: ld % 4 == 0, 32-byte aligned.
+ *   ptar_burst_reduce   from the amps of every group (group g's block at amps + 256 g nreal n_psr 2) and ptar_fe_sky's
+ *                       per-template maxima jmax / jargmax (group g's [nreal][Jg] block at + 256 g nreal): B_tmpl[r][j] and
+ *                       B_tmpl_sky[r][j] (their copy in bank order), B_max[r] = max_j, argmax_tmpl / argmax_sky (ties to the
+ *                       lower template, then the lower sky index), fap[r] = e^-B (1 + B) and amp[r][4] = -M4^-1 N4 at that
+ *                       cell (add_burst's h+ = a0 g cos + a1 g sin, hx = a2 g cos + a3 g sin at psi = 0).  Per (r, a) over
+ *                       the templates a sees: Bt_max[r][a] = max 1/2 |X^|^2, argmax_psr, fap_psr = e^-Bt and, when amp_psr
+ *                       is not NULL, amp_psr[r][a][2] = M_a^-1 N_a (add_noise_transient's waveform = a0 g cos + a1 g sin); a
+ *                       pulsar that sees no template gets -inf, index -1 and NaN.  bt_maps != NULL also writes every
+ *                       1/2 |X^|^2 [nreal][n_psr][n_tmpl].
+ * Outputs are bit-identical whatever nreal, chunking or real0 produced the rows. */
+#define PTAR_BURST_MAX_TEMPLATE 4096   /* templates of a bank */
+#define PTAR_BURST_GROUP 256           /* templates per ptar_burst_project / ptar_fe_sky call: PTAR_FP_MAX_FREQ */
+#define PTAR_BURST_TB 16               /* templates per CTA of ptar_burst_project (blk holds one range per block) */
+typedef struct {
+  int32_t n_psr;              /* 2 .. PTAR_FE_MAX_PSR                                                              */
+  int32_t n_tmpl;             /* J: 1 .. PTAR_BURST_MAX_TEMPLATE                                                   */
+  int32_t n_zc;               /* z columns per pulsar: 2 n_freq of the z projection's ptar_fp_model                */
+  int32_t n_run;              /* N^-1 runs on the packed axis                                                      */
+  int32_t n_sky;              /* S, as ptar_fe_model                                                               */
+  int32_t n_sb;               /* ceil(S / 32)                                                                      */
+  const double* t;            /* [ld] MJD 86400 of every TOA                                                       */
+  const double* dinv;         /* [ld] 1 / white variance                                                           */
+  const int64_t* run_start;   /* [n_run] packed index of the run's first TOA                                       */
+  const int32_t* run_len;     /* [n_run]                                                                           */
+  const double* run_coef;     /* [n_run] e^2 / (1 + e^2 sum 1/d) of the run's ECORR e (0 without)                  */
+  const int32_t* toa_run;     /* [ld] run of every TOA, -1 in alignment slots                                      */
+  const double* tmpl;         /* [J][4]: t0 [s], 1 / tau, 2 f0, 0                                                  */
+  const int32_t* win;         /* [n_psr][J][2]: window [lo, hi) of local TOA indices (lo = hi: empty)              */
+  const int32_t* blk;         /* [n_psr][ceil(J / 16)][2]: union of the block's windows, lo a multiple of 4        */
+  const double* H;            /* [n_psr][J][2][n_zc]: H_a(j)^T, zero past the pulsar's rank                        */
+  const double* wl;           /* [n_psr][J][3]: L^-1 packed (00, 10, 11); zero for an unseen cell                  */
+  const double* Lf;           /* [J][n_psr][3]: l11, l21, l22 of M_a(j); zero for an unseen cell                   */
+  const double* linv;         /* [J][32 n_sb][10]: L4^-1 of M4(j, s) as ptar_fe_model.linv                         */
+  const double* antenna;      /* [n_psr][n_sky][2]: e_a(s) = (F+, Fx)                                              */
+  const uint8_t* seen;        /* [n_psr][J]: 1 where pulsar a sees template j                                      */
+  const int32_t* psr_order;   /* [n_psr] pulsars in grid order (descending TOA count)                              */
+  const int64_t* seg_off;     /* [n_psr] packed index of the pulsar's first TOA (multiple of 4)                    */
+} ptar_burst_model;
+
+/* y: [nreal][ld]. */
+int ptar_burst_ninv(const double* rows, int64_t ld, int32_t nreal, const ptar_burst_model* bm, double* y, void* stream);
+/* z: [nreal][n_psr][n_zc] (ptar_fp_project); amps: [nreal][n_psr][2 Jg] of group `group`. */
+int ptar_burst_project(const double* y, int64_t ld, int32_t nreal, const double* z, const ptar_burst_model* bm, int32_t group,
+                       double* amps, void* stream);
+/* amps: every group's block; jmax, jargmax: every group's [nreal][Jg] block; B_tmpl, B_tmpl_sky: [nreal][J]; B_max, fap,
+ * argmax_tmpl, argmax_sky: [nreal]; amp: [nreal][4]; Bt_max, fap_psr, argmax_psr: [nreal][n_psr]; amp_psr: [nreal][n_psr][2]
+ * or NULL; bt_maps: [nreal][n_psr][J] or NULL. */
+int ptar_burst_reduce(const double* amps, const double* jmax, const int64_t* jargmax, int32_t nreal, const ptar_burst_model* bm,
+                      double* B_tmpl, int64_t* B_tmpl_sky, double* B_max, int64_t* argmax_tmpl, int64_t* argmax_sky,
+                      double* fap, double* amp, double* Bt_max, int64_t* argmax_psr, double* fap_psr, double* amp_psr,
+                      double* bt_maps, void* stream);
 
 /* Common uncorrelated red process (CURN) likelihood on an (A, gamma) grid (csrc/ptar_curn.cuh), from the X of
  * ptar_os_project run with a ptar_os_model that holds only the projection fields (tiles, tile0, n_tile, C, nc, ncp).

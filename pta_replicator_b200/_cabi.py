@@ -52,7 +52,8 @@ EXPORTS = ("ptar_version", "ptar_last_error", "ptar_cholesky_lower", "ptar_fouri
            "ptar_run_job_tm", "ptar_run_job_to_host_tm", "ptar_os_project", "ptar_os_project_stage", "ptar_os_pairs",
            "ptar_os_null", "ptar_os_null_stage", "ptar_os_aniso", "ptar_os_aniso_stage", "ptar_os_pf", "ptar_fp_project", "ptar_fp_reduce",
            "ptar_fp_reduce_fap", "ptar_fe_sky", "ptar_fe_combine", "ptar_curn_grid", "ptar_curn_reduce",
-           "ptar_hd_grid", "ptar_rn_grid", "ptar_bwm_sky", "ptar_bwm_combine", "ptar_fs_grid")
+           "ptar_hd_grid", "ptar_rn_grid", "ptar_bwm_sky", "ptar_bwm_combine", "ptar_fs_grid",
+           "ptar_burst_ninv", "ptar_burst_project", "ptar_burst_reduce")
 OS_MAX_NC, OS_MAX_ORF, OS_MAX_PSR = 32, 4, 256     # optimal statistic: GW-basis columns, templates, pulsars (ptar.h)
 OS_MAX_NULL = 65536                                # null columns of ptar_os_null (PTAR_OS_MAX_NULL)
 OS_NULL_PHASE_SHIFT, OS_NULL_SKY_SCRAMBLE = 1, 2
@@ -66,6 +67,7 @@ HD_MAX_N, HD_JB = 4096, 32                         # HD likelihood: n_psr 2K eig
 RN_MAX_NC = 64                                     # red-noise likelihood: basis columns of ptar_rn_grid / ptar_os_project
 BWM_MAX_EPOCH = 512                                # burst-with-memory search: burst epochs (PTAR_BWM_MAX_EPOCH)
 FS_MAX_PSR, FS_MAX_BIN, FS_JB = 256, 32, 32       # free-spectrum likelihood: pulsars, bins, eigen-rows per block (ptar.h)
+BURST_MAX_TEMPLATE, BURST_GROUP, BURST_TB = 4096, 256, 16   # burst search: templates, per group, per CTA (ptar.h)
 BWM_LINV = 6                                       # packed L2^-1 doubles per (epoch pair, sky point) (csrc/ptar_bwm.cuh)
 
 
@@ -144,6 +146,13 @@ class BwmModel(C.Structure):
     _fields_ = [("n_psr", C.c_int32), ("n_t0", C.c_int32), ("n_sky", C.c_int32), ("n_sb", C.c_int32),
                 ("kp", C.c_int32), ("reserved", C.c_int32), ("sqm", C.c_void_p), ("seen", C.c_void_p), ("ant", C.c_void_p),
                 ("antenna", C.c_void_p), ("linv", C.c_void_p)]
+
+
+class BurstModel(C.Structure):
+    _fields_ = [("n_psr", C.c_int32), ("n_tmpl", C.c_int32), ("n_zc", C.c_int32), ("n_run", C.c_int32),
+                ("n_sky", C.c_int32), ("n_sb", C.c_int32)] + [
+        (k, C.c_void_p) for k in ("t", "dinv", "run_start", "run_len", "run_coef", "toa_run", "tmpl", "win", "blk", "H",
+                                  "wl", "Lf", "linv", "antenna", "seen", "psr_order", "seg_off")]
 
 
 class CurnModel(C.Structure):
@@ -230,6 +239,9 @@ def lib():
     L.ptar_fe_combine.argtypes = [vp, vp, C.c_int32, vp, vp, vp, vp, vp]
     L.ptar_bwm_sky.argtypes = [vp, C.c_int32, vp, vp, vp, vp, vp]                        # bw: address of a BwmModel
     L.ptar_bwm_combine.argtypes = [vp, vp, vp, C.c_int32, vp] + [vp] * 10 + [vp]
+    L.ptar_burst_ninv.argtypes = [vp, i64, C.c_int32, vp, vp, vp]                     # bm: address of a BurstModel
+    L.ptar_burst_project.argtypes = [vp, i64, C.c_int32, vp, vp, C.c_int32, vp, vp]
+    L.ptar_burst_reduce.argtypes = [vp, vp, vp, C.c_int32, vp] + [vp] * 12 + [vp]
     L.ptar_curn_grid.argtypes = [vp, C.c_int32, vp, vp, vp]                           # cm: address of a CurnModel
     L.ptar_curn_reduce.argtypes = [vp, C.c_int32, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     L.ptar_hd_grid.argtypes = [vp, C.c_int32, vp, vp, vp]                             # hm: address of an HdModel

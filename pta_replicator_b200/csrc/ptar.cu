@@ -9,6 +9,7 @@
 #include <algorithm>
 
 #include "../../include/ptar.h"
+#include "ptar_burst.cuh"
 #include "ptar_bwm.cuh"
 #include "ptar_curn.cuh"
 #include "ptar_generate.cuh"
@@ -931,6 +932,66 @@ int ptar_bwm_combine(const double* amps, const double* t0max, const int64_t* t0a
   ptar::bwm_psr_kernel<<<static_cast<unsigned>((n + T - 1) / T), T, 0, st>>>(amps, nreal, *bw, psr_max, psr_argmax_t0,
                                                                             psr_slope, psr_fap);
   return check_launch("ptar_bwm_combine (pulsar term)");
+}
+
+static int burst_model_check(const ptar_burst_model* bm, const char* what) {
+  if (!bm->t || !bm->dinv || !bm->run_start || !bm->run_len || !bm->run_coef || !bm->toa_run || !bm->tmpl || !bm->win || !bm->blk || !bm->H ||
+      !bm->wl || !bm->Lf || !bm->linv || !bm->antenna || !bm->seen || !bm->psr_order || !bm->seg_off)
+    return fail(-2, "%s: model arrays missing", what);
+  if (bm->n_psr < 2 || bm->n_psr > PTAR_FE_MAX_PSR || bm->n_tmpl < 1 || bm->n_tmpl > PTAR_BURST_MAX_TEMPLATE ||
+      bm->n_zc < 2 || (bm->n_zc & 1) || bm->n_run < 1)
+    return fail(-2, "%s: need 2 <= n_psr <= 128, 1 <= n_tmpl <= 4096, an even n_zc >= 2 and n_run >= 1", what);
+  if (bm->n_sky < 1 || bm->n_sky > PTAR_FE_MAX_SKY || bm->n_sb != (bm->n_sky + ptar::FE_SB - 1) / ptar::FE_SB)
+    return fail(-2, "%s: need 1 <= n_sky <= 12288 and n_sb = ceil(n_sky / 32)", what);
+  if ((reinterpret_cast<uintptr_t>(bm->win) | reinterpret_cast<uintptr_t>(bm->blk)) & 7)
+    return fail(-2, "%s: win and blk must be 8-byte aligned", what);
+  return 0;
+}
+
+int ptar_burst_ninv(const double* rows, int64_t ld, int32_t nreal, const ptar_burst_model* bm, double* y, void* stream) {
+  if (!rows || !bm || !y || nreal <= 0 || ld <= 0) return fail(-1, "ptar_burst_ninv: bad argument%s");
+  if (int rc = burst_model_check(bm, "ptar_burst_ninv")) return rc;
+  const dim3 grid(static_cast<unsigned>((ld + ptar::BU_NINV_THREADS - 1) / ptar::BU_NINV_THREADS),
+                  static_cast<unsigned>(std::min(nreal, 65535)));
+  ptar::burst_ninv_kernel<<<grid, ptar::BU_NINV_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(rows, ld, nreal, *bm, y);
+  return check_launch("ptar_burst_ninv");
+}
+
+int ptar_burst_project(const double* y, int64_t ld, int32_t nreal, const double* z, const ptar_burst_model* bm, int32_t group,
+                       double* amps, void* stream) {
+  if (!y || !z || !bm || !amps || nreal <= 0 || ld <= 0) return fail(-1, "ptar_burst_project: bad argument%s");
+  if (int rc = burst_model_check(bm, "ptar_burst_project")) return rc;
+  if (group < 0 || group * PTAR_BURST_GROUP >= bm->n_tmpl) return fail(-2, "ptar_burst_project: group out of range%s");
+  if ((ld & 3) || (reinterpret_cast<uintptr_t>(y) & 31) || (reinterpret_cast<uintptr_t>(amps) & 15))
+    return fail(-2, "ptar_burst_project: y must be 32-byte aligned with ld %% 4 == 0, amps 16-byte aligned%s");
+  const int jg = std::min(PTAR_BURST_GROUP, bm->n_tmpl - group * PTAR_BURST_GROUP);
+  const int64_t blocks =
+      int64_t(bm->n_psr) * ((nreal + ptar::OS_RB - 1) / ptar::OS_RB) * ((jg + ptar::BU_TB - 1) / ptar::BU_TB);
+  if (blocks > 0x7fffffff) return fail(-3, "ptar_burst_project: grid too large%s");
+  static SmemOptIn optin;
+  if (int rc = opt_in_smem(ptar::burst_project_kernel, optin, ptar::BU_SMEM, "ptar_burst_project")) return rc;
+  ptar::burst_project_kernel<<<static_cast<unsigned>(blocks), ptar::BU_THREADS, ptar::BU_SMEM,
+                               static_cast<cudaStream_t>(stream)>>>(y, ld, nreal, z, *bm, group, amps);
+  return check_launch("ptar_burst_project");
+}
+
+int ptar_burst_reduce(const double* amps, const double* jmax, const int64_t* jargmax, int32_t nreal, const ptar_burst_model* bm,
+                      double* B_tmpl, int64_t* B_tmpl_sky, double* B_max, int64_t* argmax_tmpl, int64_t* argmax_sky,
+                      double* fap, double* amp, double* Bt_max, int64_t* argmax_psr, double* fap_psr, double* amp_psr,
+                      double* bt_maps, void* stream) {
+  if (!amps || !jmax || !jargmax || !bm || !B_tmpl || !B_tmpl_sky || !B_max || !argmax_tmpl || !argmax_sky || !fap || !amp ||
+      !Bt_max || !argmax_psr || !fap_psr || nreal <= 0)
+    return fail(-1, "ptar_burst_reduce: bad argument%s");
+  if (int rc = burst_model_check(bm, "ptar_burst_reduce")) return rc;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int T = ptar::BU_REDUCE_THREADS;
+  ptar::burst_reduce_kernel<<<static_cast<unsigned>((nreal + T - 1) / T), T, 0, st>>>(
+      amps, jmax, jargmax, nreal, *bm, B_tmpl, B_tmpl_sky, B_max, argmax_tmpl, argmax_sky, fap, amp);
+  if (int rc = check_launch("ptar_burst_reduce")) return rc;
+  const int64_t n = int64_t(nreal) * bm->n_psr;
+  ptar::burst_psr_kernel<<<static_cast<unsigned>((n + T - 1) / T), T, 0, st>>>(amps, nreal, *bm, Bt_max, argmax_psr, fap_psr,
+                                                                             amp_psr, bt_maps);
+  return check_launch("ptar_burst_reduce (per pulsar)");
 }
 
 static int curn_grid_check(const ptar_curn_model* cm, const char* what) {

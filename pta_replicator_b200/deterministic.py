@@ -96,15 +96,15 @@ def _inject(psr, name, params, seconds):
     psr.update_residuals()
 
 
-def add_burst(psr, gwtheta, gwphi, waveform_plus, waveform_cross, psi=0.0, tref=0, remove_quad=False, signal_name="burst"):
-    """GW burst of arbitrary waveform with elliptical polarisation -- drop-in for ``add_burst``
-    (deterministic.py:718-793).  The two waveform callables are evaluated on the host (they are the caller's Python
-    functions of ``t - tref`` [s], as in the reference); the polarisation mix and antenna projection run in
-    ``ptar_burst_delay``.  ``remove_quad`` fits the quadratic out with ``np.polyfit`` like the reference (:777-779)."""
+def burst_delay(psr, gwtheta, gwphi, waveform_plus, waveform_cross, psi=0.0, tref=0, remove_quad=False, device=None):
+    """The delay [s] ``add_burst`` adds to ``psr``, in its TOA table order: the two waveform callables of ``t - tref``
+    [s] evaluated on the host (as in the reference), the polarisation mix and antenna projection in ``ptar_burst_delay``
+    on ``device`` (default the current CUDA device) and, with ``remove_quad``, the quadratic fitted out by ``np.polyfit``
+    as the reference does (:777-779)."""
     import torch
 
     from . import _cabi
-    dev = _cabi.require_cuda()
+    dev = _cabi.require_cuda() if device is None else device
     fplus, fcross = _antenna(psr, gwtheta, gwphi)
     toas = np.asarray(psr.toas.get_mjds().value, dtype=np.float64) * 86400 - tref
     def sample(w):  # a scalar-valued callable broadcasts like numpy would in the reference
@@ -112,24 +112,39 @@ def add_burst(psr, gwtheta, gwphi, waveform_plus, waveform_cross, psi=0.0, tref=
 
     hp, hx = sample(waveform_plus), sample(waveform_cross)
     out = torch.empty(len(toas), dtype=torch.float64, device=dev)
-    _cabi.check(_cabi.lib().ptar_burst_delay(out.data_ptr(), hp.data_ptr(), hx.data_ptr(), fplus, fcross, float(np.cos(2 * psi)),
-                                             float(np.sin(2 * psi)), 0, len(toas), _cabi.current_stream()), "ptar_burst_delay")
+    with torch.cuda.device(dev):
+        _cabi.check(_cabi.lib().ptar_burst_delay(out.data_ptr(), hp.data_ptr(), hx.data_ptr(), fplus, fcross,
+                                                 float(np.cos(2 * psi)), float(np.sin(2 * psi)), 0, len(toas),
+                                                 _cabi.current_stream()), "ptar_burst_delay")
     res = out.cpu().numpy()
     if remove_quad:
         pp = np.polyfit(toas, res, 2)
         res = res - pp[0] * toas ** 2 - pp[1] * toas - pp[2]
+    return res
+
+
+def add_burst(psr, gwtheta, gwphi, waveform_plus, waveform_cross, psi=0.0, tref=0, remove_quad=False, signal_name="burst"):
+    """GW burst of arbitrary waveform with elliptical polarisation -- drop-in for ``add_burst``
+    (deterministic.py:718-793): the delay of ``burst_delay``."""
+    res = burst_delay(psr, gwtheta, gwphi, waveform_plus, waveform_cross, psi, tref, remove_quad)
     _inject(psr, "{}_".format(psr.name) + signal_name,
             {"gwtheta": gwtheta, "gwphi": gwphi, "waveform_plus": waveform_plus, "waveform_cross": waveform_cross, "psi": psi,
              "tref": tref, "remove_quad": remove_quad}, res)
+
+
+def noise_transient_delay(psr, waveform, tref=0):
+    """The delay [s] ``add_noise_transient`` adds to ``psr``, in its TOA table order: the caller's callable sampled at
+    ``t - tref`` [s] (t = MJD 86400)."""
+    toas = np.asarray(psr.toas.get_mjds().value, dtype=np.float64) * 86400 - tref
+    return np.array(np.broadcast_to(np.asarray(waveform(toas), dtype=np.float64), toas.shape))
 
 
 def add_noise_transient(psr, waveform, tref=0, signal_name="noise_transient"):
     """Incoherent transient of arbitrary waveform in one pulsar -- drop-in for ``add_noise_transient``
     (deterministic.py:796-819).  The delay IS the caller's callable sampled at ``t - tref``; there is no arithmetic to
     move to the device, so this is ledger bookkeeping only."""
-    toas = np.asarray(psr.toas.get_mjds().value, dtype=np.float64) * 86400 - tref
-    res = np.array(np.broadcast_to(np.asarray(waveform(toas), dtype=np.float64), toas.shape))
-    _inject(psr, "{}_".format(psr.name) + signal_name, {"waveform": waveform, "tref": tref}, res)
+    _inject(psr, "{}_".format(psr.name) + signal_name, {"waveform": waveform, "tref": tref},
+            noise_transient_delay(psr, waveform, tref))
 
 
 def add_gw_memory(psr, strain, gwtheta, gwphi, bwm_pol, t0_mjd, signal_name="gw_memory"):
