@@ -59,6 +59,9 @@
  *   ptar_fs_grid           no counterpart (an MCMC over enterprise's free_spectrum model per realization): the
  *                          factorised free-spectrum likelihood, one log10 rho grid per GW frequency bin, uncorrelated or
  *                          ORF-correlated, reduced by ptar_curn_reduce
+ *   ptar_fs_y2 /           no counterpart (a refit of a spectral model to the free spectrum per realization, as
+ *   ptar_fs_refit          ceffyl does from KDEs): power-law, turnover or user spectra on a grid, exact in the factorised
+ *                          per-bin likelihoods, reduced by ptar_curn_reduce
  *   ptar_bwm_sky /         no counterpart (a matched-filter search of add_gw_memory's ramp per realization): the
  *   ptar_bwm_combine       coherent burst-with-memory statistic over epoch x sky and the pulsar-term statistic, reduced
  *                          on the device
@@ -89,7 +92,8 @@ extern "C" {
                              search (ptar_bwm_model, ptar_bwm_sky, ptar_bwm_combine, PTAR_BWM_MAX_EPOCH) and the
                              free-spectrum likelihood (ptar_fs_model, ptar_fs_grid, PTAR_FS_MAX_PSR / _BIN / _JB) and the sine-Gaussian
                              burst search (ptar_burst_model, ptar_burst_ninv, ptar_burst_project, ptar_burst_reduce,
-                             PTAR_BURST_MAX_TEMPLATE / _GROUP / _TB) are new symbols only, so
+                             PTAR_BURST_MAX_TEMPLATE / _GROUP / _TB) and the free spectrum's spectral refit
+                             (ptar_fs_refit_model, ptar_fs_y2, ptar_fs_refit, PTAR_FS_MAX_TEMPLATE) are new symbols only, so
                              a caller detects them by looking the symbol up.  ptar_os_project accepts nc up to
                              PTAR_RN_MAX_NC since the red-noise likelihood; nothing changes for nc <= PTAR_OS_MAX_NC. */
 
@@ -767,6 +771,34 @@ typedef struct {
 
 /* lnL: [nreal][n_bin][n_amp]. */
 int ptar_fs_grid(const double* X, int32_t nreal, const ptar_fs_model* fm, double* lnL, void* stream);
+
+/* Spectral refit of the factorised free spectrum (csrc/ptar_fs_refit.cuh): for a spectral model on a grid of n_tmpl
+ * templates t, each with a GW variance rho_k(t)^2 per Fourier coefficient in every bin k of a free-spectrum model
+ * (a ptar_fs_model, uncorrelated or ORF-correlated), the sum over the bins of its per-bin log-likelihood ratios,
+ *   lnL[r][t] = sum_k ln L_k(rho_k(t)) = 1/2 sum_k sum_j w_kj(t) y_kj^2 - 1/2 ldet[t],
+ *   w_kj(t) = rho_k(t)^2 / (1 + rho_k(t)^2 lambda_kj),  y_k = V_k X_k[r],  ldet[t] = sum_k sum_j log1p(rho_k(t)^2 lambda_kj),
+ * exact for the factorised model at any rho (no interpolation in a log10 rho grid).
+ *   ptar_fs_y2     y2[r][k][j] = (V_k X_k[r])_j^2 for j < np (0 past 2 n_psr) with the ptar_fs_model fm (reads n_psr, ncp,
+ *                  n_bin, n2p, np and V), the first GEMM of ptar_fs_grid.  X: [nreal][n_psr][ncp], 32-byte aligned;
+ *                  y2: [nreal][n_bin][np], 16-byte aligned.
+ *   ptar_fs_refit  lnL[r][t] from y2: one GEMM of depth n_bin np on the fp64 tensor cores, W formed on the fly, the
+ *                  depth in (k, j) index order.  lnL: [nreal][n_tmpl].
+ * A model grid (x [Nx], y [Ny]) is laid out t = i_y Nx + i_x, so its summaries are ptar_curn_reduce's with a
+ * ptar_curn_model carrying only that grid (log10_A = x, gamma = y, n_amp = Nx, n_gamma = Ny).  Outputs are
+ * bit-identical whatever nreal, chunking or real0. */
+#define PTAR_FS_MAX_TEMPLATE 65536   /* templates: the 256 x 256 grid of ptar_curn_reduce */
+typedef struct {
+  int32_t n_bin;              /* K, 1 .. PTAR_FS_MAX_BIN                                                           */
+  int32_t np;                 /* the np of the ptar_fs_model: 2 n_psr rounded up to a multiple of PTAR_FS_JB       */
+  int32_t n_tmpl;             /* 1 .. PTAR_FS_MAX_TEMPLATE                                                         */
+  int32_t reserved;
+  const double* lam;          /* [n_bin][np]: the ptar_fs_model's eigenvalues (>= 0), zero past 2 n_psr            */
+  const double* rho2;         /* [n_bin][n_tmpl] rho_k(t)^2 (finite, >= 0)                                         */
+  const double* ldet;         /* [n_tmpl]                                                                          */
+} ptar_fs_refit_model;
+
+int ptar_fs_y2(const double* X, int32_t nreal, const ptar_fs_model* fm, double* y2, void* stream);
+int ptar_fs_refit(const double* y2, int32_t nreal, const ptar_fs_refit_model* rm, double* lnL, void* stream);
 
 /* End-to-end job: GWB mix + synth + generate for realizations [real0, real0+nreal), then
  * (ptar_run_job_to_host) copy the residuals to pinned host memory, chunk by chunk, with the

@@ -53,7 +53,7 @@ EXPORTS = ("ptar_version", "ptar_last_error", "ptar_cholesky_lower", "ptar_fouri
            "ptar_os_null", "ptar_os_null_stage", "ptar_os_aniso", "ptar_os_aniso_stage", "ptar_os_pf", "ptar_fp_project", "ptar_fp_reduce",
            "ptar_fp_reduce_fap", "ptar_fe_sky", "ptar_fe_combine", "ptar_curn_grid", "ptar_curn_reduce",
            "ptar_hd_grid", "ptar_rn_grid", "ptar_bwm_sky", "ptar_bwm_combine", "ptar_fs_grid",
-           "ptar_burst_ninv", "ptar_burst_project", "ptar_burst_reduce")
+           "ptar_burst_ninv", "ptar_burst_project", "ptar_burst_reduce", "ptar_fs_y2", "ptar_fs_refit")
 OS_MAX_NC, OS_MAX_ORF, OS_MAX_PSR = 32, 4, 256     # optimal statistic: GW-basis columns, templates, pulsars (ptar.h)
 OS_MAX_NULL = 65536                                # null columns of ptar_os_null (PTAR_OS_MAX_NULL)
 OS_NULL_PHASE_SHIFT, OS_NULL_SKY_SCRAMBLE = 1, 2
@@ -67,6 +67,7 @@ HD_MAX_N, HD_JB = 4096, 32                         # HD likelihood: n_psr 2K eig
 RN_MAX_NC = 64                                     # red-noise likelihood: basis columns of ptar_rn_grid / ptar_os_project
 BWM_MAX_EPOCH = 512                                # burst-with-memory search: burst epochs (PTAR_BWM_MAX_EPOCH)
 FS_MAX_PSR, FS_MAX_BIN, FS_JB = 256, 32, 32       # free-spectrum likelihood: pulsars, bins, eigen-rows per block (ptar.h)
+FS_MAX_TEMPLATE = 65536                            # spectral refit: templates of one model (PTAR_FS_MAX_TEMPLATE)
 BURST_MAX_TEMPLATE, BURST_GROUP, BURST_TB = 4096, 256, 16   # burst search: templates, per group, per CTA (ptar.h)
 BWM_LINV = 6                                       # packed L2^-1 doubles per (epoch pair, sky point) (csrc/ptar_bwm.cuh)
 
@@ -180,6 +181,11 @@ class FsModel(C.Structure):
                 ("ldet", C.c_void_p)]
 
 
+class FsRefitModel(C.Structure):
+    _fields_ = [("n_bin", C.c_int32), ("np", C.c_int32), ("n_tmpl", C.c_int32), ("reserved", C.c_int32),
+                ("lam", C.c_void_p), ("rho2", C.c_void_p), ("ldet", C.c_void_p)]
+
+
 _lib = None
 
 
@@ -247,6 +253,8 @@ def lib():
     L.ptar_hd_grid.argtypes = [vp, C.c_int32, vp, vp, vp]                             # hm: address of an HdModel
     L.ptar_rn_grid.argtypes = [vp, C.c_int32, vp, vp, vp]                             # rm: address of an RnModel
     L.ptar_fs_grid.argtypes = [vp, C.c_int32, vp, vp, vp]                             # fm: address of an FsModel
+    L.ptar_fs_y2.argtypes = [vp, C.c_int32, vp, vp, vp]
+    L.ptar_fs_refit.argtypes = [vp, C.c_int32, vp, vp, vp]                            # rm: address of an FsRefitModel
     for name in EXPORTS:
         if name not in ("ptar_version", "ptar_last_error"):
             getattr(L, name).restype = C.c_int

@@ -19,6 +19,7 @@
 #include "ptar_fe.cuh"
 #include "ptar_fp.cuh"
 #include "ptar_fs.cuh"
+#include "ptar_fs_refit.cuh"
 #include "ptar_os.cuh"
 #include "ptar_os_aniso.cuh"
 #include "ptar_os_null.cuh"
@@ -1227,6 +1228,41 @@ int ptar_fs_grid(const double* X, int32_t nreal, const ptar_fs_model* fm, double
   if (int rc = opt_in_smem(ptar::fs_grid_kernel, optin, ptar::FS_SMEM, "ptar_fs_grid")) return rc;
   ptar::fs_grid_kernel<<<grid, ptar::FS_THREADS, ptar::FS_SMEM, static_cast<cudaStream_t>(stream)>>>(X, nreal, *fm, lnL);
   return check_launch("ptar_fs_grid");
+}
+
+int ptar_fs_y2(const double* X, int32_t nreal, const ptar_fs_model* fm, double* y2, void* stream) {
+  if (!X || !fm || !y2 || nreal <= 0) return fail(-1, "ptar_fs_y2: bad argument%s");
+  if (!fm->V) return fail(-2, "ptar_fs_y2: model arrays missing%s");
+  if (fm->n_psr < 1 || fm->n_psr > PTAR_FS_MAX_PSR || fm->n_bin < 1 || fm->n_bin > PTAR_FS_MAX_BIN ||
+      !nc_ok(2 * fm->n_bin, fm->ncp, PTAR_RN_MAX_NC))
+    return fail(-2, "ptar_fs_y2: need 1 <= n_psr <= 256, 1 <= n_bin <= 32 and ncp = 2 n_bin rounded up to a multiple of 8%s");
+  if (fm->n2p != ((2 * fm->n_psr + 7) & ~7) || fm->np != (2 * fm->n_psr + PTAR_FS_JB - 1) / PTAR_FS_JB * PTAR_FS_JB)
+    return fail(-2, "ptar_fs_y2: need n2p = 2 n_psr rounded up to a multiple of 8 and np to a multiple of 32%s");
+  if ((reinterpret_cast<uintptr_t>(X) & 31) || (reinterpret_cast<uintptr_t>(fm->V) & 15) ||
+      (reinterpret_cast<uintptr_t>(y2) & 15))
+    return fail(-2, "ptar_fs_y2: X must be 32-byte aligned, V and y2 16-byte aligned%s");
+  const int64_t nrb = (int64_t(nreal) + ptar::FS_RB - 1) / ptar::FS_RB;
+  const dim3 grid(static_cast<unsigned>(nrb), static_cast<unsigned>(fm->n_bin));
+  static SmemOptIn optin;
+  if (int rc = opt_in_smem(ptar::fs_y2_kernel, optin, ptar::FS_Y2_SMEM, "ptar_fs_y2")) return rc;
+  ptar::fs_y2_kernel<<<grid, ptar::FS_THREADS, ptar::FS_Y2_SMEM, static_cast<cudaStream_t>(stream)>>>(X, nreal, *fm, y2);
+  return check_launch("ptar_fs_y2");
+}
+
+int ptar_fs_refit(const double* y2, int32_t nreal, const ptar_fs_refit_model* rm, double* lnL, void* stream) {
+  if (!y2 || !rm || !lnL || nreal <= 0) return fail(-1, "ptar_fs_refit: bad argument%s");
+  if (!rm->lam || !rm->rho2 || !rm->ldet) return fail(-2, "ptar_fs_refit: model arrays missing%s");
+  if (rm->n_bin < 1 || rm->n_bin > PTAR_FS_MAX_BIN || rm->np < PTAR_FS_JB || rm->np > 2 * PTAR_FS_MAX_PSR ||
+      rm->np % PTAR_FS_JB || rm->n_tmpl < 1 || rm->n_tmpl > PTAR_FS_MAX_TEMPLATE)
+    return fail(-2, "ptar_fs_refit: need 1 <= n_bin <= 32, np a multiple of 32 in 32 .. 512 and 1 <= n_tmpl <= 65536%s");
+  if (reinterpret_cast<uintptr_t>(y2) & 15) return fail(-2, "ptar_fs_refit: y2 must be 16-byte aligned%s");
+  const int64_t nrb = (int64_t(nreal) + ptar::RF_RB - 1) / ptar::RF_RB;
+  if (nrb > 65535) return fail(-3, "ptar_fs_refit: more than 65535 realization blocks%s");
+  const dim3 grid(static_cast<unsigned>((rm->n_tmpl + ptar::RF_TB - 1) / ptar::RF_TB), static_cast<unsigned>(nrb));
+  static SmemOptIn optin;
+  if (int rc = opt_in_smem(ptar::fs_refit_kernel, optin, ptar::RF_SMEM, "ptar_fs_refit")) return rc;
+  ptar::fs_refit_kernel<<<grid, ptar::RF_THREADS, ptar::RF_SMEM, static_cast<cudaStream_t>(stream)>>>(y2, nreal, *rm, lnL);
+  return check_launch("ptar_fs_refit");
 }
 
 }  // extern "C"
