@@ -93,7 +93,9 @@ extern "C" {
                              free-spectrum likelihood (ptar_fs_model, ptar_fs_grid, PTAR_FS_MAX_PSR / _BIN / _JB) and the sine-Gaussian
                              burst search (ptar_burst_model, ptar_burst_ninv, ptar_burst_project, ptar_burst_reduce,
                              PTAR_BURST_MAX_TEMPLATE / _GROUP / _TB) and the free spectrum's spectral refit
-                             (ptar_fs_refit_model, ptar_fs_y2, ptar_fs_refit, PTAR_FS_MAX_TEMPLATE) are new symbols only, so
+                             (ptar_fs_refit_model, ptar_fs_y2, ptar_fs_refit, PTAR_FS_MAX_TEMPLATE) and chromatic noise in
+                             the generator (ptar_chrom_model, ptar_generate_chrom, ptar_generate_stage_chrom,
+                             ptar_run_job_to_host_chrom, PTAR_K_CHROM, PTAR_CHROM_SLOTS) are new symbols only, so
                              a caller detects them by looking the symbol up.  ptar_os_project accepts nc up to
                              PTAR_RN_MAX_NC since the red-noise likelihood; nothing changes for nc <= PTAR_OS_MAX_NC. */
 
@@ -117,6 +119,7 @@ extern "C" {
 #define PTAR_K_ECORR  3
 #define PTAR_K_RED    4
 #define PTAR_K_GWB    5
+#define PTAR_K_CHROM  6   /* chromatic coefficients: index = (slot << 16) | Fourier column */
 
 /* One tile of the packed TOA axis: <=1024 consecutive (time-sorted) TOAs of ONE pulsar
  * touching <=64 kernel-epochs. */
@@ -274,6 +277,32 @@ int ptar_generate(const ptar_gen_params* p, void* stream);
  * (Fourier GEMM, ECORR, GWB grid -> Cbuf), stage 2 = TOA kernel (Cbuf + white noise -> out).  ptar_generate
  * issues both; this entry exists so a caller can time them separately. */
 int ptar_generate_stage(const ptar_gen_params* p, int stage, void* stream);
+
+/* Chromatic Gaussian processes (DM variations, scattering) on top of ptar_generate: up to PTAR_CHROM_SLOTS slots, each
+ *     out[r][i] += w_s[i] * sum_j F_s(t_i)_j scale_s[psr][j] z_j
+ * with the per-TOA weight w_s[i] = (fref / nu_i)^idx_s and F_s the (sin, cos)(2 pi f t) basis on absolute time.  Like the
+ * red noise, each slot is evaluated per (kernel-epoch, realization) as a quadratic in dt (its own Fourier GEMM in the
+ * epoch stage) and the TOA stage adds w_s[i] times its Horner value; the tile's nd holds for every process.
+ * A pulsar without a slot has on_s[psr] = 0 (its weights, scales and draws are never read).  Throughput-mode
+ * coefficients are drawn on their own Philox stream (PTAR_K_CHROM, index (s << 16) | column), so every other draw is
+ * the one ptar_generate makes.  The parity mode (p->z* set) needs zchr [nreal][n_psr][J_0 + ... + J_{n_slot-1}].
+ * cm == NULL runs exactly ptar_generate / ptar_generate_stage.  With p->Cbuf the scratch must hold
+ * c_rows * ceil(nreal/rc) * (3 rc (1 + n_slot) + 2) doubles. */
+#define PTAR_CHROM_SLOTS 2
+typedef struct {
+  int32_t n_slot;                          /* 1 .. PTAR_CHROM_SLOTS                                     */
+  int32_t J[PTAR_CHROM_SLOTS];             /* basis columns of each slot (2 * components, even)         */
+  int32_t reserved;
+  const double*  Ftile[PTAR_CHROM_SLOTS];  /* [n_tiles][J_s][64]: basis at the epoch reference times    */
+  const double*  scale[PTAR_CHROM_SLOTS];  /* [n_psr][J_s] sqrt(prior)                                  */
+  const double*  omega[PTAR_CHROM_SLOTS];  /* [n_psr][J_s/2] 2*pi*f_k                                   */
+  const double*  weight[PTAR_CHROM_SLOTS]; /* [ld_out] per-TOA weight (fref / nu)^idx                   */
+  const int32_t* on[PTAR_CHROM_SLOTS];     /* [n_psr] 1 = the pulsar carries this slot                  */
+  const double*  zchr;                     /* parity mode: [nreal][n_psr][sum_s J_s] standard normals   */
+} ptar_chrom_model;
+
+int ptar_generate_chrom(const ptar_gen_params* p, const ptar_chrom_model* cm, void* stream);
+int ptar_generate_stage_chrom(const ptar_gen_params* p, const ptar_chrom_model* cm, int stage, void* stream);
 
 /* Raw throughput-mode normals (fp32 Box-Muller of Philox4x32-10), for tests:
  * out[k] = normal(kind, psr, realization, idx0 + k), k < n.  Counter = (idx, kind | psr << 8,
@@ -853,6 +882,12 @@ int ptar_run_job_tm(const ptar_job* job, const ptar_timing_model* tm, double* sc
 int ptar_run_job_to_host_tm(const ptar_job* job, const ptar_timing_model* tm, double* scratch, int64_t scratch_len,
                             int64_t real0, int64_t nreal, int32_t chunk, double* out_host, double* dev_buf0,
                             double* dev_buf1, void* stream0, void* stream1);
+
+/* ptar_run_job_to_host_tm with chromatic noise (ptar_generate_chrom); tm and cm may each be NULL, and with cm == NULL this
+ * is exactly ptar_run_job_to_host_tm.  A parity-mode cm->zchr advances with the chunks like gen.zrn. */
+int ptar_run_job_to_host_chrom(const ptar_job* job, const ptar_timing_model* tm, const ptar_chrom_model* cm, double* scratch,
+                               int64_t scratch_len, int64_t real0, int64_t nreal, int32_t chunk, double* out_host,
+                               double* dev_buf0, double* dev_buf1, void* stream0, void* stream1);
 
 #ifdef __cplusplus
 }

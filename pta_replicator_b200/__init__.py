@@ -17,7 +17,7 @@ def __getattr__(name):  # lazy: keeps `import pta_replicator_b200` free of torch
     if name in ("add_measurement_noise", "add_jitter", "add_efac", "add_ecorr", "quantize_fast"):
         from . import white_noise
         return getattr(white_noise, name)
-    if name in ("add_red_noise", "add_gwb", "create_fourier_design_matrix_red"):
+    if name in ("add_red_noise", "add_gwb", "create_fourier_design_matrix_red", "add_dm_noise", "add_chromatic_noise"):
         from . import red_noise
         return getattr(red_noise, name)
     if name in ("add_cgw", "add_catalog_of_cws", "add_burst", "add_noise_transient", "add_gw_memory",

@@ -33,6 +33,15 @@ def epoch_smem_bytes(J):
     return 16 + 8 * (max(J * TILE_EPOCHS + 3 * J * EPK_RB, 3 * 24 * 64) + TILE_EPOCHS * EPK_RB * 2)
 
 
+def gen_chrom_smem_bytes(Jo, rc, n_slot, split_epoch=False):
+    """Shared memory of the chromatic generator's epoch stage (gen_chrom_smem_bytes / epoch_smem_bytes of
+    ptar_generate.cuh) for the widest basis Jo and n_slot chromatic slots; the larger of the schedule's kernels."""
+    if split_epoch and rc != 32:
+        return max(epoch_smem_bytes(Jo), 16 + 8 * TILE_EPOCHS * (3 * 16 * (1 + n_slot) + 2))
+    rc = rc or 16
+    return 16 + 8 * (max(Jo * TILE_EPOCHS + 3 * Jo * rc, TILE_EPOCHS * (3 * rc + 2)) + TILE_EPOCHS * (3 * rc * n_slot + 2))
+
+
 def max_red_columns(rc=16, split_epoch=False):
     """The largest (even) red-noise basis width J whose epoch stage fits shared memory in the given schedule: 258 fused at
     rc = 16, 180 at rc = 32 (fused or two-kernel), 154 in the two-kernel schedule's epoch kernel (rc = 16)."""
@@ -44,7 +53,8 @@ def max_red_columns(rc=16, split_epoch=False):
 
 F_WHITE, F_ECORR, F_RED, F_GWB, F_DET, F_WHITE1 = 1, 2, 4, 8, 16, 32
 TM_KMAX = 32                                       # timing-model columns per pulsar (PTAR_TM_KMAX)
-K_WHITE1, K_WHITE2, K_ECORR, K_RED, K_GWB = 1, 2, 3, 4, 5
+K_WHITE1, K_WHITE2, K_ECORR, K_RED, K_GWB, K_CHROM = 1, 2, 3, 4, 5, 6
+CHROM_SLOTS = 2                                    # chromatic slots of ptar_generate_chrom (PTAR_CHROM_SLOTS)
 
 EXPORTS = ("ptar_version", "ptar_last_error", "ptar_cholesky_lower", "ptar_fourier_basis", "ptar_cgw_delay", "ptar_cw_catalog", "ptar_burst_delay", "ptar_memory_delay",
            "ptar_gwb_mix", "ptar_gwb_synth", "ptar_gwb_mix_i8", "ptar_gwb_slice_i8", "ptar_gwb_synth_i8", "ptar_debug_i8_timestamps", "ptar_generate", "ptar_generate_stage", "ptar_philox_normals", "ptar_peer_export", "ptar_peer_open", "ptar_peer_close", "ptar_peer_copy", "ptar_run_job",
@@ -53,7 +63,8 @@ EXPORTS = ("ptar_version", "ptar_last_error", "ptar_cholesky_lower", "ptar_fouri
            "ptar_os_null", "ptar_os_null_stage", "ptar_os_aniso", "ptar_os_aniso_stage", "ptar_os_pf", "ptar_fp_project", "ptar_fp_reduce",
            "ptar_fp_reduce_fap", "ptar_fe_sky", "ptar_fe_combine", "ptar_curn_grid", "ptar_curn_reduce",
            "ptar_hd_grid", "ptar_rn_grid", "ptar_bwm_sky", "ptar_bwm_combine", "ptar_fs_grid",
-           "ptar_burst_ninv", "ptar_burst_project", "ptar_burst_reduce", "ptar_fs_y2", "ptar_fs_refit")
+           "ptar_burst_ninv", "ptar_burst_project", "ptar_burst_reduce", "ptar_fs_y2", "ptar_fs_refit",
+           "ptar_generate_chrom", "ptar_generate_stage_chrom", "ptar_run_job_to_host_chrom")
 OS_MAX_NC, OS_MAX_ORF, OS_MAX_PSR = 32, 4, 256     # optimal statistic: GW-basis columns, templates, pulsars (ptar.h)
 OS_MAX_NULL = 65536                                # null columns of ptar_os_null (PTAR_OS_MAX_NULL)
 OS_NULL_PHASE_SHIFT, OS_NULL_SKY_SCRAMBLE = 1, 2
@@ -95,12 +106,18 @@ class GenParams(C.Structure):
     ]
 
 
+class ChromModel(C.Structure):
+    _fields_ = [("n_slot", C.c_int32), ("J", C.c_int32 * CHROM_SLOTS), ("reserved", C.c_int32)] + [
+        (k, C.c_void_p * CHROM_SLOTS) for k in ("Ftile", "scale", "omega", "weight", "on")] + [("zchr", C.c_void_p)]
+
+
 class Job(C.Structure):
     _fields_ = [("gen", GenParams), ("M", C.c_void_p), ("A", C.c_void_p), ("lda", C.c_int64), ("Jg", C.c_int32),
                 ("lower_tri", C.c_int32), ("tile_list", C.c_void_p), ("knots", C.c_void_p), ("n_syn_tiles", C.c_int32),
                 ("reserved", C.c_int32), ("Zm", C.c_void_p), ("Gbuf", C.c_void_p), ("gwb_zin", C.c_void_p),
                 ("AS", C.c_void_p), ("colscale", C.c_void_p), ("ZS", C.c_void_p), ("zscale", C.c_void_p), ("zinv", C.c_void_p),
                 ("tile_list_i8", C.c_void_p), ("rcap", C.c_int64), ("Jpad", C.c_int32), ("n_syn_tiles_i8", C.c_int32)]
+    chrom = None   # the engine's ChromModel of the job (not part of the C struct): None without chromatic noise
 
 
 class TimingModel(C.Structure):
@@ -255,6 +272,10 @@ def lib():
     L.ptar_fs_grid.argtypes = [vp, C.c_int32, vp, vp, vp]                             # fm: address of an FsModel
     L.ptar_fs_y2.argtypes = [vp, C.c_int32, vp, vp, vp]
     L.ptar_fs_refit.argtypes = [vp, C.c_int32, vp, vp, vp]                            # rm: address of an FsRefitModel
+    L.ptar_generate_chrom.argtypes = [C.POINTER(GenParams), C.POINTER(ChromModel), vp]
+    L.ptar_generate_stage_chrom.argtypes = [C.POINTER(GenParams), C.POINTER(ChromModel), i32, vp]
+    L.ptar_run_job_to_host_chrom.argtypes = [C.POINTER(Job), vp, C.POINTER(ChromModel), vp, i64, i64, i64, C.c_int32, vp, vp,
+                                             vp, vp, vp]
     for name in EXPORTS:
         if name not in ("ptar_version", "ptar_last_error"):
             getattr(L, name).restype = C.c_int

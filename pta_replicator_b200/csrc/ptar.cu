@@ -262,56 +262,108 @@ __global__ void philox_normals_kernel(float* __restrict__ out, int kind, int psr
   out[k] = z[realization & 3];
 }
 
-template <int RC, bool INJECT, int WHITE, int DET, int STAGE>
-int launch_stage(const ptar_gen_params& p, cudaStream_t st) {
+// Widest GEMM operand of a chromatic build: red noise or any slot.
+int chrom_jo(const ptar_gen_params& p, const ptar_chrom_model* cm) {
+  int jo = (p.flags & PTAR_F_RED) ? p.J : 0;
+  for (int s = 0; s < cm->n_slot; ++s) jo = std::max(jo, int(cm->J[s]));
+  return jo;
+}
+
+template <int RC, bool INJECT, int WHITE, int DET, int STAGE, int CHROM = 0>
+int launch_stage(const ptar_gen_params& p, cudaStream_t st, const ptar_chrom_model* cm = nullptr) {
   // STAGE 2 only needs the Cs block; STAGE 0/1 need the GEMM operands
   size_t smem = ptar::gen_smem_bytes(p.J, RC);
   if (STAGE == 2) smem = 16 + sizeof(double) * ptar::EP * ptar::gen_css(RC);
-  if (smem > 227 * 1024) return fail(-3, "ptar_generate: J too large for shared memory%s");
+  if (CHROM) smem = ptar::gen_chrom_smem_bytes(chrom_jo(p, cm), RC, cm->n_slot, STAGE);
+  if (smem > 227 * 1024)
+    return fail(-3, CHROM ? "ptar_generate_chrom: red-noise and chromatic bases too wide for shared memory at this rc%s"
+                          : "ptar_generate: J too large for shared memory%s");
   static SmemOptIn optin;  // per instantiation
-  if (int rc = opt_in_smem(ptar::gen_kernel<RC, INJECT, WHITE, DET, STAGE>, optin, 227 * 1024, "ptar_generate")) return rc;
+  if constexpr (CHROM) {
+    if (int rc = opt_in_smem(ptar::gen_chrom_kernel<RC, INJECT, WHITE, DET, STAGE>, optin, 227 * 1024, "ptar_generate_chrom"))
+      return rc;
+  } else {
+    if (int rc = opt_in_smem(ptar::gen_kernel<RC, INJECT, WHITE, DET, STAGE>, optin, 227 * 1024, "ptar_generate")) return rc;
+  }
   const dim3 grid((p.nreal + RC - 1) / RC, p.n_tiles);
   if (grid.y > 65535) return fail(-3, "ptar_generate: more than 65535 tiles%s");
   if (STAGE != 0 && p.Cbuf) {  // the Cs blocks of this build must fit the scratch the caller gave
-    const int64_t need = p.c_rows * int64_t(grid.x) * ptar::gen_css(RC);
+    const int64_t need = p.c_rows * int64_t(grid.x) * (ptar::gen_css(RC) + (CHROM ? 3 * RC * cm->n_slot : 0));
     if (p.c_rows <= 0 || p.cbuf_len < need) return fail(-2, "ptar_generate: Cbuf too small for this rc (need c_rows * ceil(nreal/rc) * (3 rc + 2) doubles)%s");
   }
-  ptar::gen_kernel<RC, INJECT, WHITE, DET, STAGE><<<grid, ptar::gen_threads(RC), smem, st>>>(p, ptar::philox_keys(p.seed));
-  return check_launch("ptar_generate");
+  if constexpr (CHROM) {
+    ptar::gen_chrom_kernel<RC, INJECT, WHITE, DET, STAGE><<<grid, ptar::gen_threads(RC), smem, st>>>(p, ptar::philox_keys(p.seed), *cm);
+    return check_launch("ptar_generate_chrom");
+  } else {
+    ptar::gen_kernel<RC, INJECT, WHITE, DET, STAGE><<<grid, ptar::gen_threads(RC), smem, st>>>(p, ptar::philox_keys(p.seed));
+    return check_launch("ptar_generate");
+  }
 }
 
 // Epoch kernel of the two-kernel schedule (RC = 16 blocks of Cbuf, two per CTA).
-template <bool INJECT>
-int launch_epoch(const ptar_gen_params& p, cudaStream_t st) {
-  const size_t smem = ptar::epoch_smem_bytes(p.J);
-  if (smem > 227 * 1024) return fail(-3, "ptar_generate: J too large for shared memory%s");
+template <bool INJECT, int CHROM = 0>
+int launch_epoch(const ptar_gen_params& p, cudaStream_t st, const ptar_chrom_model* cm = nullptr) {
+  const size_t smem = ptar::epoch_smem_bytes(CHROM ? chrom_jo(p, cm) : p.J);
+  if (smem > 227 * 1024)
+    return fail(-3, CHROM ? "ptar_generate_chrom: red-noise and chromatic bases too wide for the epoch kernel%s"
+                          : "ptar_generate: J too large for shared memory%s");
   static SmemOptIn optin;
-  if (int rc = opt_in_smem(ptar::epoch_kernel<INJECT>, optin, 227 * 1024, "ptar_generate (epoch kernel)")) return rc;
   const dim3 grid((p.nreal + ptar::EPK_RB - 1) / ptar::EPK_RB, p.n_tiles);
   if (grid.y > 65535) return fail(-3, "ptar_generate: more than 65535 tiles%s");
   {
-    const int64_t need = p.c_rows * int64_t((p.nreal + 15) / 16) * ptar::EPK_CSS;
+    const int64_t need = p.c_rows * int64_t((p.nreal + 15) / 16) * (ptar::EPK_CSS + (CHROM ? 48 * cm->n_slot : 0));
     if (p.c_rows <= 0 || p.cbuf_len < need) return fail(-2, "ptar_generate: Cbuf too small (need c_rows * ceil(nreal/16) * 50 doubles)%s");
   }
-  ptar::epoch_kernel<INJECT><<<grid, ptar::EPK_THREADS, smem, st>>>(p, ptar::philox_keys(p.seed));
-  return check_launch("ptar_generate (epoch kernel)");
+  if constexpr (CHROM) {
+    if (int rc = opt_in_smem(ptar::epoch_chrom_kernel<INJECT>, optin, 227 * 1024, "ptar_generate_chrom (epoch kernel)")) return rc;
+    ptar::epoch_chrom_kernel<INJECT><<<grid, ptar::EPK_THREADS, smem, st>>>(p, ptar::philox_keys(p.seed), *cm);
+    return check_launch("ptar_generate_chrom (epoch kernel)");
+  } else {
+    if (int rc = opt_in_smem(ptar::epoch_kernel<INJECT>, optin, 227 * 1024, "ptar_generate (epoch kernel)")) return rc;
+    ptar::epoch_kernel<INJECT><<<grid, ptar::EPK_THREADS, smem, st>>>(p, ptar::philox_keys(p.seed));
+    return check_launch("ptar_generate (epoch kernel)");
+  }
 }
 
 thread_local int g_only_stage = 0;  // set by ptar_generate_stage: 1 = epoch kernel only, 2 = TOA kernel only
 
-template <int RC, bool INJECT, int WHITE, int DET>
-int launch_gen(const ptar_gen_params& p, cudaStream_t st) {
-  const bool has_epoch = (p.flags & (PTAR_F_RED | PTAR_F_ECORR | PTAR_F_GWB)) != 0;
+template <int RC, bool INJECT, int WHITE, int DET, int CHROM = 0>
+int launch_gen(const ptar_gen_params& p, cudaStream_t st, const ptar_chrom_model* cm = nullptr) {
+  const bool has_epoch = CHROM || (p.flags & (PTAR_F_RED | PTAR_F_ECORR | PTAR_F_GWB)) != 0;
   if (p.Cbuf && has_epoch) {  // two-kernel schedule
     if (g_only_stage != 2) {
       // the epoch kernel does not depend on WHITE / DET
-      const int rc = RC == 16 ? launch_epoch<INJECT>(p, st) : launch_stage<RC, INJECT, -1, -1, 1>(p, st);
+      const int rc = RC == 16 ? launch_epoch<INJECT, CHROM>(p, st, cm) : launch_stage<RC, INJECT, -1, -1, 1, CHROM>(p, st, cm);
       if (rc || g_only_stage == 1) return rc;
     }
-    return launch_stage<RC, INJECT, WHITE, DET, 2>(p, st);
+    return launch_stage<RC, INJECT, WHITE, DET, 2, CHROM>(p, st, cm);
   }
   if (g_only_stage == 1) return 0;   // nothing to do: no epoch terms (or fused schedule)
-  return launch_stage<RC, INJECT, WHITE, DET, 0>(p, st);
+  return launch_stage<RC, INJECT, WHITE, DET, 0, CHROM>(p, st, cm);
+}
+
+// The build for (parity mode | rc, white draws, deterministic term).
+template <int CHROM>
+int dispatch_gen(const ptar_gen_params& p, cudaStream_t st, const ptar_chrom_model* cm, bool inject, int rc, int white, bool det) {
+  if (inject) return launch_gen<16, true, -1, -1, CHROM>(p, st, cm);
+  if (rc == 32) {
+    switch (white * 2 + (det ? 1 : 0)) {
+      case 0: return launch_gen<32, false, 0, 0, CHROM>(p, st, cm);
+      case 1: return launch_gen<32, false, 0, 1, CHROM>(p, st, cm);
+      case 2: return launch_gen<32, false, 1, 0, CHROM>(p, st, cm);
+      case 3: return launch_gen<32, false, 1, 1, CHROM>(p, st, cm);
+      case 4: return launch_gen<32, false, 2, 0, CHROM>(p, st, cm);
+      default: return launch_gen<32, false, 2, 1, CHROM>(p, st, cm);
+    }
+  }
+  switch (white * 2 + (det ? 1 : 0)) {
+    case 0: return launch_gen<16, false, 0, 0, CHROM>(p, st, cm);
+    case 1: return launch_gen<16, false, 0, 1, CHROM>(p, st, cm);
+    case 2: return launch_gen<16, false, 1, 0, CHROM>(p, st, cm);
+    case 3: return launch_gen<16, false, 1, 1, CHROM>(p, st, cm);
+    case 4: return launch_gen<16, false, 2, 0, CHROM>(p, st, cm);
+    default: return launch_gen<16, false, 2, 1, CHROM>(p, st, cm);
+  }
 }
 
 template <bool INJECT, bool SLICE>
@@ -508,7 +560,9 @@ int ptar_debug_i8_timestamps(void* buf) {
   return 0;
 }
 
-int ptar_generate(const ptar_gen_params* pp, void* stream) {
+int ptar_generate(const ptar_gen_params* pp, void* stream) { return ptar_generate_chrom(pp, nullptr, stream); }
+
+int ptar_generate_chrom(const ptar_gen_params* pp, const ptar_chrom_model* cm, void* stream) {
   if (!pp) return fail(-1, "ptar_generate: null params%s");
   const ptar_gen_params& p = *pp;
   if (!p.out || !p.tiles || p.n_tiles <= 0 || p.nreal <= 0 || p.n_psr <= 0)
@@ -525,7 +579,7 @@ int ptar_generate(const ptar_gen_params* pp, void* stream) {
   if ((p.flags & PTAR_F_GWB) && ((p.g_ldr & 3) || p.g_ldr < ((p.nreal + 3) & ~3) || (reinterpret_cast<uintptr_t>(p.G) & 31)))
     return fail(-2, "ptar_generate: G must be 32-byte aligned, column-major with g_ldr %% 4 == 0 >= nreal rounded up to 4%s");
   if ((p.flags & PTAR_F_DET) && !p.det) return fail(-2, "ptar_generate: DET needs det%s");
-  const bool inject = p.z1 || p.z2 || p.zb || p.zrn;
+  const bool inject = p.z1 || p.z2 || p.zb || p.zrn || (cm && cm->zchr);
   if (inject) {
     if ((p.flags & PTAR_F_WHITE) && (!p.z1 || (!(p.flags & PTAR_F_WHITE1) && !p.z2))) return fail(-2, "ptar_generate: injected white draws missing%s");
     if ((p.flags & PTAR_F_ECORR) && (!p.zb || !p.psr_bucket_off)) return fail(-2, "ptar_generate: injected ECORR draws missing%s");
@@ -534,37 +588,33 @@ int ptar_generate(const ptar_gen_params* pp, void* stream) {
     return fail(-2, "ptar_generate: real0 must be a multiple of 4%s");
   }
   if (p.Cbuf && p.cbuf_len <= 0) return fail(-2, "ptar_generate: Cbuf given without cbuf_len%s");
+  if (cm) {
+    if (cm->n_slot < 1 || cm->n_slot > PTAR_CHROM_SLOTS) return fail(-2, "ptar_generate_chrom: n_slot must be 1 or 2%s");
+    for (int s = 0; s < cm->n_slot; ++s) {
+      if (cm->J[s] <= 0 || (cm->J[s] & 1) || !cm->Ftile[s] || !cm->scale[s] || !cm->omega[s] || !cm->weight[s] || !cm->on[s])
+        return fail(-2, "ptar_generate_chrom: every slot needs even J > 0, Ftile, scale, omega, weight and on%s");
+    }
+    if (!p.eloc || !p.dtau) return fail(-2, "ptar_generate_chrom: chromatic terms need eloc/dtau%s");
+    if (inject && !cm->zchr) return fail(-2, "ptar_generate_chrom: injected chromatic draws missing%s");
+  }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int rc = p.rc ? p.rc : 16;
   if (rc != 16 && rc != 32) return fail(-2, "ptar_generate: rc must be 16 or 32%s");
-  if (inject) return launch_gen<16, true, -1, -1>(p, st);
   const int white = !(p.flags & PTAR_F_WHITE) ? 0 : ((p.flags & PTAR_F_WHITE1) ? 1 : 2);
   const bool det = (p.flags & PTAR_F_DET) != 0;
-  if (rc == 32) {
-    switch (white * 2 + (det ? 1 : 0)) {
-      case 0: return launch_gen<32, false, 0, 0>(p, st);
-      case 1: return launch_gen<32, false, 0, 1>(p, st);
-      case 2: return launch_gen<32, false, 1, 0>(p, st);
-      case 3: return launch_gen<32, false, 1, 1>(p, st);
-      case 4: return launch_gen<32, false, 2, 0>(p, st);
-      default: return launch_gen<32, false, 2, 1>(p, st);
-    }
-  }
-  switch (white * 2 + (det ? 1 : 0)) {
-    case 0: return launch_gen<16, false, 0, 0>(p, st);
-    case 1: return launch_gen<16, false, 0, 1>(p, st);
-    case 2: return launch_gen<16, false, 1, 0>(p, st);
-    case 3: return launch_gen<16, false, 1, 1>(p, st);
-    case 4: return launch_gen<16, false, 2, 0>(p, st);
-    default: return launch_gen<16, false, 2, 1>(p, st);
-  }
+  if (cm) return dispatch_gen<1>(p, st, cm, inject, rc, white, det);
+  return dispatch_gen<0>(p, st, nullptr, inject, rc, white, det);
 }
 
 int ptar_generate_stage(const ptar_gen_params* pp, int stage, void* stream) {
+  return ptar_generate_stage_chrom(pp, nullptr, stage, stream);
+}
+
+int ptar_generate_stage_chrom(const ptar_gen_params* pp, const ptar_chrom_model* cm, int stage, void* stream) {
   if (stage < 1 || stage > 2) return fail(-1, "ptar_generate_stage: stage must be 1 (epoch kernel) or 2 (TOA kernel)%s");
   if (!pp || !pp->Cbuf) return fail(-2, "ptar_generate_stage: needs the two-kernel schedule (Cbuf)%s");
   g_only_stage = stage;
-  const int rc = ptar_generate(pp, stream);
+  const int rc = ptar_generate_chrom(pp, cm, stream);
   g_only_stage = 0;
   return rc;
 }
@@ -1109,14 +1159,22 @@ int ptar_rn_grid(const double* X, int32_t nreal, const ptar_rn_model* rm, double
   return check_launch("ptar_rn_grid");
 }
 
+static int run_job(const ptar_job* job, const ptar_timing_model* tm, const ptar_chrom_model* cm, double* scratch,
+                   int64_t scratch_len, int64_t real0, int32_t nreal, double* out, void* stream);
+
 int ptar_run_job_tm(const ptar_job* job, const ptar_timing_model* tm, double* scratch, int64_t scratch_len, int64_t real0,
                     int32_t nreal, double* out, void* stream) {
+  return run_job(job, tm, nullptr, scratch, scratch_len, real0, nreal, out, stream);
+}
+
+static int run_job(const ptar_job* job, const ptar_timing_model* tm, const ptar_chrom_model* cm, double* scratch,
+                   int64_t scratch_len, int64_t real0, int32_t nreal, double* out, void* stream) {
   if (!job || !out || nreal <= 0) return fail(-1, "ptar_run_job: bad argument%s");
   ptar_gen_params g = job->gen;
   g.real0 = real0;
   g.nreal = nreal;
   g.out = out;
-  const bool inject = g.z1 || g.z2 || g.zb || g.zrn || job->gwb_zin;
+  const bool inject = g.z1 || g.z2 || g.zb || g.zrn || job->gwb_zin || (cm && cm->zchr);
   if (g.flags & PTAR_F_GWB) {
     if (!job->M || !job->A || !job->Zm || !job->Gbuf || !job->tile_list || !job->knots)
       return fail(-2, "ptar_run_job: GWB buffers missing%s");
@@ -1144,7 +1202,7 @@ int ptar_run_job_tm(const ptar_job* job, const ptar_timing_model* tm, double* sc
     if (rc) return rc;
     g.G = job->Gbuf;
   }
-  if (int rc = ptar_generate(&g, stream)) return rc;
+  if (int rc = ptar_generate_chrom(&g, cm, stream)) return rc;
   if (tm) return ptar_timing_project(out, g.ld_out, nreal, tm, scratch, scratch_len, stream);
   return 0;
 }
@@ -1156,6 +1214,13 @@ int ptar_run_job(const ptar_job* job, int64_t real0, int32_t nreal, double* out,
 int ptar_run_job_to_host_tm(const ptar_job* job, const ptar_timing_model* tm, double* scratch, int64_t scratch_len,
                             int64_t real0, int64_t nreal, int32_t chunk, double* out_host, double* dev_buf0,
                             double* dev_buf1, void* stream0, void* stream1) {
+  return ptar_run_job_to_host_chrom(job, tm, nullptr, scratch, scratch_len, real0, nreal, chunk, out_host, dev_buf0, dev_buf1,
+                                    stream0, stream1);
+}
+
+int ptar_run_job_to_host_chrom(const ptar_job* job, const ptar_timing_model* tm, const ptar_chrom_model* cm, double* scratch,
+                               int64_t scratch_len, int64_t real0, int64_t nreal, int32_t chunk, double* out_host,
+                               double* dev_buf0, double* dev_buf1, void* stream0, void* stream1) {
   if (!job || !out_host || !dev_buf0 || !dev_buf1 || chunk <= 0 || (chunk & 3) || nreal <= 0)
     return fail(-1, "ptar_run_job_to_host: bad argument (chunk must be a positive multiple of 4)%s");
   cudaStream_t s0 = static_cast<cudaStream_t>(stream0), s1 = static_cast<cudaStream_t>(stream1);
@@ -1183,7 +1248,14 @@ int ptar_run_job_to_host_tm(const ptar_job* job, const ptar_timing_model* tm, do
     if (j.gen.zb) j.gen.zb += done * j.gen.n_bucket_total;
     if (j.gen.zrn) j.gen.zrn += done * int64_t(j.gen.n_psr) * j.gen.J;
     if (j.gwb_zin) j.gwb_zin += done * int64_t(j.gen.n_psr) * j.Jg;
-    rc = ptar_run_job_tm(&j, tm, scratch, scratch_len, real0 + done, n, bufs[b], s0);
+    ptar_chrom_model cmc;
+    if (cm) {
+      cmc = *cm;
+      int zld = 0;
+      for (int s = 0; s < cmc.n_slot && s < PTAR_CHROM_SLOTS; ++s) zld += cmc.J[s];
+      if (cmc.zchr) cmc.zchr += done * int64_t(j.gen.n_psr) * zld;
+    }
+    rc = run_job(&j, tm, cm ? &cmc : nullptr, scratch, scratch_len, real0 + done, n, bufs[b], s0);
     if (rc) break;
     if (!ok(cudaEventRecord(gen_done[b], s0)) || !ok(cudaStreamWaitEvent(s1, gen_done[b], 0))) break;
     if (!ok(cudaMemcpyAsync(out_host + done * ld, bufs[b], sizeof(double) * size_t(n) * ld, cudaMemcpyDeviceToHost, s1))) break;

@@ -5,6 +5,7 @@
 //             + sum_j F(t_i)_j sqrt(prior_j) z_j       red_noise.py:126-128
 //             + lerp(G[r][psr], t_i)                   red_noise.py:286-287
 //             + det_i                                  deterministic.py:160-165
+//             + sum_s w_s(i) sum_j F(t_i)_j sqrt(prior_s,j) z_j    chromatic slots (DM, scattering; CHROM builds)
 //
 // One CTA = one tile (<=1024 time-sorted TOAs of one pulsar, <=64 kernel-epochs) x RC
 // realizations.  Everything that is smooth inside an epoch is evaluated once per
@@ -60,15 +61,14 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
 // ---- pieces of the epoch stage shared by the fused kernel (gen_body) and the standalone epoch kernel: one copy of
 // the arithmetic, so the two schedules agree bit for bit by construction.
 
-// Red-noise coefficients a = sqrt(prior) * z of RB realizations and their first two time derivatives (1/2 folded into
-// the 2nd): As = [3][J][RB].  One work item = one (even, odd) column pair x 4 realizations (red_noise.py:126-127).
-template <int RB, bool INJECT, int NTHREADS>
-__device__ __forceinline__ void rn_coefficients(const ptar_gen_params& P, const PhiloxKeys& K, uint32_t psr, int J, int r0,
-                                                int nr, uint64_t rgroup0, double* As, int tid) {
+// Fourier-process coefficients a = sqrt(prior) * z of RB realizations and their first two time derivatives (1/2 folded
+// into the 2nd): As = [3][J][RB].  One work item = one (even, odd) column pair x 4 realizations (red_noise.py:126-127).
+// zrow(r) = the injected draws of local realization r (parity mode); Philox index blk0 + column on stream ``kind``.
+template <int RB, bool INJECT, int NTHREADS, class ZRow>
+__device__ __forceinline__ void fourier_coefficients(const double* scale, const double* om, double sgn_even, ZRow zrow,
+                                                     uint32_t kind, uint32_t blk0, const PhiloxKeys& K, uint32_t psr, int J,
+                                                     int nr, uint64_t rgroup0, double* As, int tid) {
   constexpr int RG = RB / 4;
-  const double* scale = P.rn_scale + size_t(psr) * J;
-  const double* om = P.rn_omega + size_t(psr) * (J / 2);
-  const double sgn_even = P.rn_convention ? 1.0 : -1.0;
   double* A0 = As;
   double* A1 = As + size_t(J) * RB;
   double* A2 = As + size_t(2) * J * RB;
@@ -81,16 +81,16 @@ __device__ __forceinline__ void rn_coefficients(const ptar_gen_params& P, const 
       for (int l = 0; l < 4; ++l) {
         const int r = rg * 4 + l;
         const bool ok = r < nr;
-        const size_t zi = (size_t(r0 + (ok ? r : 0)) * P.n_psr + psr) * J;
-        ye[l] = ok ? P.zrn[zi + je] : 0.0;
-        yo[l] = ok ? P.zrn[zi + jo] : 0.0;
+        const double* z = zrow(ok ? r : 0);
+        ye[l] = ok ? z[je] : 0.0;
+        yo[l] = ok ? z[jo] : 0.0;
       }
     } else {
       float n[4];
-      normals4(n, je, PTAR_K_RED, psr, rgroup0 + rg, K);
+      normals4(n, blk0 + je, kind, psr, rgroup0 + rg, K);
 #pragma unroll
       for (int l = 0; l < 4; ++l) ye[l] = static_cast<double>(n[l]);
-      normals4(n, jo, PTAR_K_RED, psr, rgroup0 + rg, K);
+      normals4(n, blk0 + jo, kind, psr, rgroup0 + rg, K);
 #pragma unroll
       for (int l = 0; l < 4; ++l) yo[l] = static_cast<double>(n[l]);
     }
@@ -115,6 +115,67 @@ __device__ __forceinline__ void rn_coefficients(const ptar_gen_params& P, const 
     put(A2 + je * RB, h * ae[0], h * ae[1], h * ae[2], h * ae[3]);
     put(A2 + jo * RB, h * ao[0], h * ao[1], h * ao[2], h * ao[3]);
   }
+}
+
+// Red-noise coefficients of RB realizations (first local realization r0).
+template <int RB, bool INJECT, int NTHREADS>
+__device__ __forceinline__ void rn_coefficients(const ptar_gen_params& P, const PhiloxKeys& K, uint32_t psr, int J, int r0,
+                                                int nr, uint64_t rgroup0, double* As, int tid) {
+  auto zrow = [&](int r) { return P.zrn + (size_t(r0 + r) * P.n_psr + psr) * J; };
+  fourier_coefficients<RB, INJECT, NTHREADS>(P.rn_scale + size_t(psr) * J, P.rn_omega + size_t(psr) * (J / 2),
+                                             P.rn_convention ? 1.0 : -1.0, zrow, PTAR_K_RED, 0u, K, psr, J, nr, rgroup0, As,
+                                             tid);
+}
+
+// Coefficients of chromatic slot s (basis (sin, cos) on absolute time, as rn_convention = 0); zoff = first column of
+// the slot in the injected zchr rows.
+template <int RB, bool INJECT, int NTHREADS>
+__device__ __forceinline__ void chrom_coefficients(const ptar_gen_params& P, const ptar_chrom_model& CM, const PhiloxKeys& K,
+                                                   int s, int zoff, int zld, uint32_t psr, int r0, int nr, uint64_t rgroup0,
+                                                   double* As, int tid) {
+  const int J = CM.J[s];
+  auto zrow = [&](int r) { return CM.zchr + (size_t(r0 + r) * P.n_psr + psr) * zld + zoff; };
+  fourier_coefficients<RB, INJECT, NTHREADS>(CM.scale[s] + size_t(psr) * J, CM.omega[s] + size_t(psr) * (J / 2), -1.0, zrow,
+                                             PTAR_K_CHROM, uint32_t(s) << 16, K, psr, J, nr, rgroup0, As, tid);
+}
+
+// One bulk-async copy global -> shared completing on mbarrier ``bar``, and the wait for phase ``parity`` of ``bar``.
+__device__ __forceinline__ void bulk_to_smem(uint64_t* bar, double* dst, const double* src, uint32_t bytes) {
+  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(dst)),
+               "l"(src), "r"(bytes), "r"(smem_u32(bar))
+               : "memory");
+}
+
+__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
+  uint32_t done = 0;
+  while (!done) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
+        "selp.u32 %0, 1, 0, p;\n\t}"
+        : "=r"(done)
+        : "r"(smem_u32(bar)), "r"(parity)
+        : "memory");
+  }
+}
+
+__device__ __forceinline__ void mbar_init(uint64_t* bar) {
+  asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_u32(bar)));
+  asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+}
+
+// Shared memory of the chromatic builds: the operands of the widest GEMM (Jo columns) or the red-noise block Cs[64][css]
+// that aliases them, then the chromatic block Cx[64][3 RC n_slot + 2] of the slots' sums.  The TOA-only kernel (STAGE 2)
+// holds one unified block [64][3 RC (1 + n_slot) + 2].
+__host__ __device__ inline size_t gen_chrom_xoff(int Jo, int RC) {
+  const size_t ops = size_t(Jo) * EP + size_t(3) * Jo * RC;
+  const size_t cs = size_t(EP) * gen_css(RC);
+  return ops > cs ? ops : cs;
+}
+__host__ __device__ inline size_t gen_chrom_smem_bytes(int Jo, int RC, int n_slot, int stage) {
+  if (stage == 2) return 16 + sizeof(double) * EP * (gen_css(RC) + 3 * RC * n_slot);
+  return 16 + sizeof(double) * (gen_chrom_xoff(Jo, RC) + size_t(EP) * (3 * RC * n_slot + 2));
 }
 
 // GWB grid values of 4 consecutive realizations (first local row rl) at knot column j and j + 1: the grid is
@@ -163,6 +224,50 @@ __device__ __forceinline__ void epoch_addends4(const ptar_gen_params& P, const P
   }
 }
 
+// The quadratic of 4 realizations at dt: c = 12 doubles (c0, c1, c2) x 4 of one Cs row, nd Taylor terms.
+__device__ __forceinline__ void quad4(const double* c, double dt, int nd, double v[4]) {
+  const double2* c2 = reinterpret_cast<const double2*>(c);
+  const double2 q0 = c2[0], q1 = c2[1], q2 = c2[2], q3 = c2[3], q4 = c2[4], q5 = c2[5];
+  // (c0,c1,c2) x 4 realizations = q0.x q0.y q1.x | q1.y q2.x q2.y | q3.x q3.y q4.x | q4.y q5.x q5.y
+  if (nd > 2) {
+    v[0] = fma(dt, fma(dt, q1.x, q0.y), q0.x);
+    v[1] = fma(dt, fma(dt, q2.y, q2.x), q1.y);
+    v[2] = fma(dt, fma(dt, q4.x, q3.y), q3.x);
+    v[3] = fma(dt, fma(dt, q5.y, q5.x), q4.y);
+  } else if (nd > 1) {  // (c0, c1) only
+    v[0] = fma(dt, q0.y, q0.x);
+    v[1] = fma(dt, q2.x, q1.y);
+    v[2] = fma(dt, q3.y, q3.x);
+    v[3] = fma(dt, q5.x, q4.y);
+  } else {
+    v[0] = q0.x; v[1] = q1.y; v[2] = q3.x; v[3] = q4.y;
+  }
+}
+
+// C[e][r][d] += sum_{j in [jlo, jhi)} F[j][e] * A[d][j][r] for epochs e0..e0+3 and realization rr of the fused epoch stage
+// (F = Fs[J][64], A = As[3][J][RC]); one instantiation per Taylor order, so no predicated-off FMAs in the loop.
+template <int RC>
+__device__ __forceinline__ void epoch_gemm(const double* Fs, const double* As, int J, int jlo, int jhi, int e0, int rr, int nd,
+                                           double acc[4][3]) {
+  auto gemm = [&](auto ND) {
+    constexpr int kNd = decltype(ND)::value;
+    for (int j = jlo; j < jhi; ++j) {
+      const double2 f01 = *reinterpret_cast<const double2*>(Fs + j * EP + e0);
+      const double2 f23 = *reinterpret_cast<const double2*>(Fs + j * EP + e0 + 2);
+      const double f[4] = {f01.x, f01.y, f23.x, f23.y};
+#pragma unroll
+      for (int d = 0; d < kNd; ++d) {
+        const double a = As[(d * J + j) * RC + rr];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) acc[i][d] = fma(f[i], a, acc[i][d]);
+      }
+    }
+  };
+  if (nd >= 3) gemm(std::integral_constant<int, 3>{});
+  else if (nd == 2) gemm(std::integral_constant<int, 2>{});
+  else gemm(std::integral_constant<int, 1>{});
+}
+
 // WHITE / DET: -1 = decided at run time from P.flags (generic build, used by the parity mode);
 // WHITE 0/1/2 = no white noise / one merged draw / two draws, DET 0/1 = no / with deterministic term
 // (specialised builds of the throughput mode: the flag tests disappear from the inner loop).
@@ -170,9 +275,11 @@ __device__ __forceinline__ void epoch_addends4(const ptar_gen_params& P, const P
 // Cs[n_ep][CSS] goes to P.Cbuf; STAGE 2: TOA stage only, the block comes back with one bulk-async copy.
 // Splitting costs ~20 % extra HBM traffic but the TOA-stage warps no longer share their SM with warps that
 // sit in the epoch stage's barriers and load latencies.
-template <int RC, bool INJECT, int WHITE, int DET, int STAGE>
+// CHROM = 1: the chromatic slots of *CM (ptar_generate_chrom) -- their GEMMs run first, into Cx, so that the red-noise
+// block Cs can still alias the GEMM operands; CHROM = 0 builds never touch CM.
+template <int RC, bool INJECT, int WHITE, int DET, int STAGE, int CHROM = 0>
 __device__ __forceinline__ void gen_body(const ptar_gen_params& P, const PhiloxKeys& K, const int tile_idx,
-                                         const int chunk_idx, unsigned char* smem_raw) {
+                                         const int chunk_idx, unsigned char* smem_raw, const ptar_chrom_model* CM) {
   constexpr int GEN_THREADS = 16 * RC;
   uint64_t* mbar = reinterpret_cast<uint64_t*>(smem_raw);
   double* Fs = reinterpret_cast<double*>(smem_raw + 16);
@@ -190,14 +297,27 @@ __device__ __forceinline__ void gen_body(const ptar_gen_params& P, const PhiloxK
   const bool has_red = (flags & PTAR_F_RED) && J > 0;
   const bool has_ecorr = (flags & PTAR_F_ECORR) != 0;
   const bool has_gwb = (flags & PTAR_F_GWB) && P.npts > 0;
-  const bool has_epoch = has_red || has_ecorr || has_gwb;
+  const bool has_epoch = has_red || has_ecorr || has_gwb || CHROM > 0;
   const int nd = tile.nd;
   const uint32_t psr = static_cast<uint32_t>(tile.psr);
   const uint64_t rgroup0 = static_cast<uint64_t>(P.real0 + r0) >> 2;
+  // chromatic builds: Cbuf rows are [red 3 RC | slot 0 3 RC | slot 1 3 RC | 2 pad] (css_u doubles); in shared memory the
+  // TOA-only kernel keeps that row, the epoch stage keeps the slots apart in Cx[64][cssx]
+  const int n_slot = CHROM ? CM->n_slot : 0;
+  const int css_u = CSS + 3 * RC * n_slot;
+  const int rowp = STAGE == 2 ? css_u : CSS;
+  int Jo = J;
+  if (CHROM) {
+#pragma unroll
+    for (int s = 0; s < PTAR_CHROM_SLOTS; ++s) Jo = s < n_slot ? max(Jo, CM->J[s]) : Jo;
+  }
+  double* Cx = CHROM ? (STAGE == 2 ? Cs + 3 * RC : Fs + gen_chrom_xoff(Jo, RC)) : nullptr;
+  const int cssx = STAGE == 2 ? css_u : 3 * RC * n_slot + 2;
+  const bool on0 = CHROM && CM->on[0][psr], on1 = CHROM && n_slot > 1 && CM->on[1][psr];
 
   const int n_chunks = (P.nreal + RC - 1) / RC;
   double* cblock = (STAGE != 0 && P.Cbuf)
-                       ? P.Cbuf + (size_t(tile.reserved) * n_chunks + size_t(chunk_idx) * tile.n_ep) * CSS
+                       ? P.Cbuf + (size_t(tile.reserved) * n_chunks + size_t(chunk_idx) * tile.n_ep) * css_u
                        : nullptr;
   if (STAGE == 2) {
     if (has_epoch) {  // fetch the block the epoch kernel left for this (tile, chunk)
@@ -207,7 +327,7 @@ __device__ __forceinline__ void gen_body(const ptar_gen_params& P, const PhiloxK
       }
       __syncthreads();
       if (tid == 0) {
-        const uint32_t bytes = static_cast<uint32_t>(sizeof(double) * tile.n_ep * CSS);
+        const uint32_t bytes = static_cast<uint32_t>(sizeof(double) * tile.n_ep * css_u);
         asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(mbar)), "r"(bytes)
                      : "memory");
         asm volatile(
@@ -243,6 +363,62 @@ __device__ __forceinline__ void gen_body(const ptar_gen_params& P, const PhiloxK
 #pragma unroll
   for (int i = 0; i < 4; ++i) acc[i][0] = acc[i][1] = acc[i][2] = 0.0;
 
+  if (CHROM) {  // chromatic slots: the same GEMM over each slot's basis tile, sums to Cx
+    uint64_t* cbar = mbar + 1;
+    uint32_t phase = 0;
+    if (tid == 0) mbar_init(cbar);
+    const int zld = CM->J[0] + (n_slot > 1 ? CM->J[1] : 0);
+#pragma unroll
+    for (int s = 0; s < PTAR_CHROM_SLOTS; ++s) {
+      if (s >= n_slot) break;
+      const int zoff = s ? CM->J[0] : 0;
+      if (!(s == 0 ? on0 : on1)) continue;  // uniform per CTA
+      const int Js = CM->J[s];
+      double* Asx = Fs + size_t(Js) * EP;
+      __syncthreads();  // the previous slot's operands are consumed; cbar's init is visible
+      if (tid == 0)
+        bulk_to_smem(cbar, Fs, CM->Ftile[s] + size_t(tile_idx) * Js * EP, static_cast<uint32_t>(sizeof(double) * Js * EP));
+      chrom_coefficients<RC, INJECT, GEN_THREADS>(P, *CM, K, s, zoff, zld, psr, r0, nr, rgroup0, Asx, tid);
+      __syncthreads();
+      mbar_wait(cbar, phase);
+      phase ^= 1;
+      double cacc[4][3];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) cacc[i][0] = cacc[i][1] = cacc[i][2] = 0.0;
+      if (e0 < tile.n_ep) epoch_gemm<RC>(Fs, Asx, Js, (Js * ks) / nsplit, (Js * (ks + 1)) / nsplit, e0, rr, nd, cacc);
+      __syncthreads();  // operands consumed
+      double* cx = Cx + 3 * RC * s;
+      if (nsplit > 1) {
+        if (ks > 0) {
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            double* c = cx + (ks * eper + e0 + i) * cssx + rr * 3;
+            c[0] = cacc[i][0]; c[1] = cacc[i][1]; c[2] = cacc[i][2];
+          }
+        }
+        __syncthreads();
+        if (ks == 0) {
+          for (int g = 1; g < nsplit; ++g) {
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+              const double* c = cx + (g * eper + e0 + i) * cssx + rr * 3;
+              cacc[i][0] += c[0]; cacc[i][1] += c[1]; cacc[i][2] += c[2];
+            }
+          }
+        }
+        __syncthreads();
+      }
+      if (ks == 0) {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          double* c = cx + (e0 + i) * cssx + rr * 3;
+          c[0] = cacc[i][0]; c[1] = cacc[i][1]; c[2] = cacc[i][2];
+        }
+      }
+    }
+    __syncthreads();  // Fs is free for the red-noise tile
+  }
+
   if (has_red) {
     if (tid == 0) {
       asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_u32(mbar)));
@@ -276,26 +452,7 @@ __device__ __forceinline__ void gen_body(const ptar_gen_params& P, const PhiloxK
       }
     }
     // C[e][r][d] = sum_j F[j][e] * A[d][j][r]   (this thread: columns [jlo, jhi))
-    if (e0 < tile.n_ep) {
-      const int jlo = (J * ks) / nsplit, jhi = (J * (ks + 1)) / nsplit;
-      auto gemm = [&](auto ND) {  // one instantiation per Taylor order: no predicated-off FMAs in the loop
-        constexpr int kNd = decltype(ND)::value;
-        for (int j = jlo; j < jhi; ++j) {
-          const double2 f01 = *reinterpret_cast<const double2*>(Fs + j * EP + e0);
-          const double2 f23 = *reinterpret_cast<const double2*>(Fs + j * EP + e0 + 2);
-          const double f[4] = {f01.x, f01.y, f23.x, f23.y};
-#pragma unroll
-          for (int d = 0; d < kNd; ++d) {
-            const double a = As[(d * J + j) * RC + rr];
-#pragma unroll
-            for (int i = 0; i < 4; ++i) acc[i][d] = fma(f[i], a, acc[i][d]);
-          }
-        }
-      };
-      if (nd >= 3) gemm(std::integral_constant<int, 3>{});
-      else if (nd == 2) gemm(std::integral_constant<int, 2>{});
-      else gemm(std::integral_constant<int, 1>{});
-    }
+    if (e0 < tile.n_ep) epoch_gemm<RC>(Fs, As, J, (J * ks) / nsplit, (J * (ks + 1)) / nsplit, e0, rr, nd, acc);
     __syncthreads();  // everyone is done reading Fs / As: Cs may overwrite them
     if (nsplit > 1) {  // split-K reduction: groups ks >= 1 park their partial sums in rows ks*eper + e
       if (ks > 0) {
@@ -349,7 +506,14 @@ __device__ __forceinline__ void gen_body(const ptar_gen_params& P, const PhiloxK
   if (has_epoch) __syncthreads();
 
     if (STAGE == 1) {
-      if (has_epoch) {
+      if (CHROM) {  // red rows and slot rows merge into the Cbuf row
+        const int n = tile.n_ep * css_u;
+        for (int idx = tid; idx < n; idx += GEN_THREADS) {
+          const int e = idx / css_u, c = idx - e * css_u;
+          const double v = c < 3 * RC ? Cs[e * CSS + c] : (c < css_u - 2 ? Cx[e * cssx + c - 3 * RC] : 0.0);
+          __stcg(cblock + idx, v);
+        }
+      } else if (has_epoch) {
         const int n = tile.n_ep * CSS;
         for (int idx = tid; idx < n; idx += GEN_THREADS) __stcg(cblock + idx, Cs[idx]);
       }
@@ -369,6 +533,7 @@ __device__ __forceinline__ void gen_body(const ptar_gen_params& P, const PhiloxK
     const double det = has_det ? P.det[gi] : 0.0;
     const double dt = (has_epoch && nd > 1) ? P.dtau[gi] : 0.0;
     const int el = has_epoch ? static_cast<int>(P.eloc[gi]) : 0;
+    const double wc0 = on0 ? CM->weight[0][gi] : 0.0, wc1 = on1 ? CM->weight[1][gi] : 0.0;
     const uint32_t wblock = static_cast<uint32_t>(tile.toa_local0 + tt);
     double* orow = P.out + size_t(r0) * ld + gi;
 #pragma unroll kGenUnroll
@@ -383,21 +548,19 @@ __device__ __forceinline__ void gen_body(const ptar_gen_params& P, const PhiloxK
       }
       double v[4] = {0.0, 0.0, 0.0, 0.0};
       if (has_epoch) {
-        const double2* c2 = reinterpret_cast<const double2*>(Cs + el * CSS + rg * 12);
-        const double2 q0 = c2[0], q1 = c2[1], q2 = c2[2], q3 = c2[3], q4 = c2[4], q5 = c2[5];
-        // (c0,c1,c2) x 4 realizations = q0.x q0.y q1.x | q1.y q2.x q2.y | q3.x q3.y q4.x | q4.y q5.x q5.y
-        if (nd > 2) {
-          v[0] = fma(dt, fma(dt, q1.x, q0.y), q0.x);
-          v[1] = fma(dt, fma(dt, q2.y, q2.x), q1.y);
-          v[2] = fma(dt, fma(dt, q4.x, q3.y), q3.x);
-          v[3] = fma(dt, fma(dt, q5.y, q5.x), q4.y);
-        } else if (nd > 1) {  // (c0, c1) only
-          v[0] = fma(dt, q0.y, q0.x);
-          v[1] = fma(dt, q2.x, q1.y);
-          v[2] = fma(dt, q3.y, q3.x);
-          v[3] = fma(dt, q5.x, q4.y);
-        } else {
-          v[0] = q0.x; v[1] = q1.y; v[2] = q3.x; v[3] = q4.y;
+        quad4(Cs + el * rowp + rg * 12, dt, nd, v);
+        if (CHROM) {  // + w_s(TOA) * quadratic of slot s
+          double q[4];
+          if (on0) {
+            quad4(Cx + el * cssx + rg * 12, dt, nd, q);
+#pragma unroll
+            for (int l = 0; l < 4; ++l) v[l] = fma(wc0, q[l], v[l]);
+          }
+          if (on1) {
+            quad4(Cx + el * cssx + 3 * RC + rg * 12, dt, nd, q);
+#pragma unroll
+            for (int l = 0; l < 4; ++l) v[l] = fma(wc1, q[l], v[l]);
+          }
         }
       }
       if (has_det) {
@@ -455,7 +618,15 @@ __device__ __forceinline__ void gen_body(const ptar_gen_params& P, const PhiloxK
 template <int RC, bool INJECT, int WHITE, int DET, int STAGE>
 __global__ void __launch_bounds__(16 * RC, 1024 / (16 * RC)) gen_kernel(const ptar_gen_params P, const PhiloxKeys K) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
-  gen_body<RC, INJECT, WHITE, DET, STAGE>(P, K, blockIdx.y, blockIdx.x, smem_raw);
+  gen_body<RC, INJECT, WHITE, DET, STAGE>(P, K, blockIdx.y, blockIdx.x, smem_raw, nullptr);
+}
+
+// The same with chromatic slots.  Their Cx block leaves room for two CTAs per SM at most (RC = 16, J = 60: 79-104 KB).
+template <int RC, bool INJECT, int WHITE, int DET, int STAGE>
+__global__ void __launch_bounds__(16 * RC, 512 / (16 * RC)) gen_chrom_kernel(const ptar_gen_params P, const PhiloxKeys K,
+                                                                           const ptar_chrom_model CM) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  gen_body<RC, INJECT, WHITE, DET, STAGE, 1>(P, K, blockIdx.y, blockIdx.x, smem_raw, &CM);
 }
 
 // ---- standalone epoch kernel (two-kernel schedule) ------------------------------------------------------
@@ -477,15 +648,79 @@ __host__ __device__ inline size_t epoch_smem_bytes(int J) {
   return 16 + sizeof(double) * (ops + size_t(EP) * EPK_RB * 2);  // + Add[64][32][2]
 }
 
-template <bool INJECT>
-__global__ void __launch_bounds__(EPK_THREADS, 2) epoch_kernel(const ptar_gen_params P, const PhiloxKeys K) {
-  extern __shared__ __align__(16) unsigned char smem_raw[];
+// acc[i][l][d] += sum_{j in [jlo, jhi)} F[j][e0 + i] * A[d][j][2 rp + l] (epoch kernel: 4 epochs x 2 realizations x nd)
+__device__ __forceinline__ void epk_gemm(const double* Fs, const double* As, int J, int jlo, int jhi, int e0, int rp, int nd,
+                                         double acc[4][2][3]) {
+  auto gemm = [&](auto ND) {
+    constexpr int kNd = decltype(ND)::value;
+#pragma unroll 2
+    for (int j = jlo; j < jhi; ++j) {
+      const double2 f01 = *reinterpret_cast<const double2*>(Fs + j * EP + e0);
+      const double2 f23 = *reinterpret_cast<const double2*>(Fs + j * EP + e0 + 2);
+      const double f[4] = {f01.x, f01.y, f23.x, f23.y};
+#pragma unroll
+      for (int d = 0; d < kNd; ++d) {
+        const double2 a = *reinterpret_cast<const double2*>(As + (d * J + j) * EPK_RB + 2 * rp);
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          acc[i][0][d] = fma(f[i], a.x, acc[i][0][d]);
+          acc[i][1][d] = fma(f[i], a.y, acc[i][1][d]);
+        }
+      }
+    }
+  };
+  if (nd >= 3) gemm(std::integral_constant<int, 3>{});
+  else if (nd == 2) gemm(std::integral_constant<int, 2>{});
+  else gemm(std::integral_constant<int, 1>{});
+}
+
+// split-K of the epoch kernel: groups ks >= 1 park their 24 partial sums in scratch[ks-1][q][tg] (over the dead operands
+// at Fs), group 0 adds them in group order
+__device__ __forceinline__ void epk_split_k(double* Fs, int ks, int nsplit, int gthreads, int tg, double acc[4][2][3]) {
+  __syncthreads();
+  double* scratch = Fs;
+  if (ks > 0) {
+    double* s = scratch + size_t(ks - 1) * 24 * gthreads + tg;
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+      for (int l = 0; l < 2; ++l)
+#pragma unroll
+        for (int d = 0; d < 3; ++d) s[((i * 2 + l) * 3 + d) * gthreads] = acc[i][l][d];
+  }
+  __syncthreads();
+  if (ks == 0) {
+    for (int g = 1; g < nsplit; ++g) {
+      const double* s = scratch + size_t(g - 1) * 24 * gthreads + tg;
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int l = 0; l < 2; ++l)
+#pragma unroll
+          for (int d = 0; d < 3; ++d) acc[i][l][d] += s[((i * 2 + l) * 3 + d) * gthreads];
+    }
+  }
+}
+
+// Its chromatic build (CHROM = 1) sizes the operand region for the widest basis (Jo columns: epoch_smem_bytes(Jo)), then
+// runs one more GEMM per slot after the red-noise one, into the slot's columns of the Cbuf row (50 + 48 n_slot doubles).
+
+template <bool INJECT, int CHROM>
+__device__ __forceinline__ void epoch_body(const ptar_gen_params& P, const PhiloxKeys& K, unsigned char* smem_raw,
+                                           const ptar_chrom_model* CM) {
   uint64_t* mbar = reinterpret_cast<uint64_t*>(smem_raw);
   double* Fs = reinterpret_cast<double*>(smem_raw + 16);
   const int J = P.J;
   constexpr int RB = EPK_RB, CSS = EPK_CSS, RG = RB / 4;
+  const int n_slot = CHROM ? CM->n_slot : 0;
+  const int css_u = CSS + 48 * n_slot;
+  int Jo = J;
+  if (CHROM) {
+#pragma unroll
+    for (int s = 0; s < PTAR_CHROM_SLOTS; ++s) Jo = s < n_slot ? max(Jo, CM->J[s]) : Jo;
+  }
   double* As = Fs + size_t(J) * EP;
-  const size_t ops = size_t(J) * EP + size_t(3) * J * RB;
+  const size_t ops = size_t(Jo) * EP + size_t(3) * Jo * RB;
   double* Add = Fs + (ops < size_t(3) * 24 * 64 ? size_t(3) * 24 * 64 : ops);  // [epoch][realization][c0 add, c1 add]
 
   const int tid = threadIdx.x;
@@ -578,56 +813,8 @@ __global__ void __launch_bounds__(EPK_THREADS, 2) epoch_kernel(const ptar_gen_pa
             : "memory");
       }
     }
-    if (e0 < tile.n_ep) {
-      const int jlo = (J * ks) / nsplit, jhi = (J * (ks + 1)) / nsplit;
-      auto gemm = [&](auto ND) {
-        constexpr int kNd = decltype(ND)::value;
-#pragma unroll 2
-        for (int j = jlo; j < jhi; ++j) {
-          const double2 f01 = *reinterpret_cast<const double2*>(Fs + j * EP + e0);
-          const double2 f23 = *reinterpret_cast<const double2*>(Fs + j * EP + e0 + 2);
-          const double f[4] = {f01.x, f01.y, f23.x, f23.y};
-#pragma unroll
-          for (int d = 0; d < kNd; ++d) {
-            const double2 a = *reinterpret_cast<const double2*>(As + (d * J + j) * RB + 2 * rp);
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              acc[i][0][d] = fma(f[i], a.x, acc[i][0][d]);
-              acc[i][1][d] = fma(f[i], a.y, acc[i][1][d]);
-            }
-          }
-        }
-      };
-      if (nd >= 3) gemm(std::integral_constant<int, 3>{});
-      else if (nd == 2) gemm(std::integral_constant<int, 2>{});
-      else gemm(std::integral_constant<int, 1>{});
-    }
-    if (nsplit > 1) {
-      // split-K: groups ks >= 1 park their 24 partial sums in scratch[ks-1][q][tg] (over the dead operands)
-      __syncthreads();
-      double* scratch = Fs;
-      if (ks > 0) {
-        double* s = scratch + size_t(ks - 1) * 24 * gthreads + tg;
-#pragma unroll
-        for (int i = 0; i < 4; ++i)
-#pragma unroll
-          for (int l = 0; l < 2; ++l)
-#pragma unroll
-            for (int d = 0; d < 3; ++d) s[((i * 2 + l) * 3 + d) * gthreads] = acc[i][l][d];
-      }
-      __syncthreads();
-      if (ks == 0) {
-        for (int g = 1; g < nsplit; ++g) {
-          const double* s = scratch + size_t(g - 1) * 24 * gthreads + tg;
-#pragma unroll
-          for (int i = 0; i < 4; ++i)
-#pragma unroll
-            for (int l = 0; l < 2; ++l)
-#pragma unroll
-              for (int d = 0; d < 3; ++d) acc[i][l][d] += s[((i * 2 + l) * 3 + d) * gthreads];
-        }
-      }
-    }
+    if (e0 < tile.n_ep) epk_gemm(Fs, As, J, (J * ks) / nsplit, (J * (ks + 1)) / nsplit, e0, rp, nd, acc);
+    if (nsplit > 1) epk_split_k(Fs, ks, nsplit, gthreads, tg, acc);
   } else if (has_add) {
     finish_add();
     __syncthreads();  // Add visible
@@ -637,7 +824,7 @@ __global__ void __launch_bounds__(EPK_THREADS, 2) epoch_kernel(const ptar_gen_pa
   const int chunk = 2 * blockIdx.x + (rp >> 3);
   if (ks == 0 && chunk < n_chunks) {
     const int rl = (2 * rp) & 15;
-    double* blockp = P.Cbuf + (size_t(tile.reserved) * n_chunks + size_t(chunk) * tile.n_ep) * CSS;
+    double* blockp = P.Cbuf + (size_t(tile.reserved) * n_chunks + size_t(chunk) * tile.n_ep) * css_u;
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       const int e = e0 + i;
@@ -648,14 +835,71 @@ __global__ void __launch_bounds__(EPK_THREADS, 2) epoch_kernel(const ptar_gen_pa
           const double2 t0 = q[0], t1 = q[1];
           a00 = t0.x; a01 = t0.y; a10 = t1.x; a11 = t1.y;
         }
-        double2* o = reinterpret_cast<double2*>(blockp + size_t(e) * CSS + rl * 3);
+        double2* o = reinterpret_cast<double2*>(blockp + size_t(e) * css_u + rl * 3);
         __stcg(o, make_double2(acc[i][0][0] + a00, acc[i][0][1] + a01));
         __stcg(o + 1, make_double2(acc[i][0][2], acc[i][1][0] + a10));
         __stcg(o + 2, make_double2(acc[i][1][1] + a11, acc[i][1][2]));
-        if (rl == 14) __stcg(o + 3, make_double2(0.0, 0.0));  // row padding (doubles 48, 49)
+        if (rl == 14) {  // row padding (the row's last two doubles)
+          if (CHROM) __stcg(reinterpret_cast<double2*>(blockp + size_t(e) * css_u + css_u - 2), make_double2(0.0, 0.0));
+          else __stcg(o + 3, make_double2(0.0, 0.0));
+        }
       }
     }
   }
+  if (CHROM) {  // one more GEMM per chromatic slot, same ownership and split-K as the red noise (same sums as gen_body)
+    uint64_t* cbar = mbar + 1;
+    uint32_t phase = 0;
+    if (tid == 0) mbar_init(cbar);
+    const int zld = CM->J[0] + (n_slot > 1 ? CM->J[1] : 0);
+#pragma unroll
+    for (int s = 0; s < PTAR_CHROM_SLOTS; ++s) {
+      if (s >= n_slot) break;
+      const int zoff = s ? CM->J[0] : 0;
+      if (!CM->on[s][psr]) continue;  // uniform per CTA
+      const int Js = CM->J[s];
+      double* Asx = Fs + size_t(Js) * EP;
+      __syncthreads();  // Fs and the split-K scratch are free; cbar's init is visible
+      if (tid == 0)
+        bulk_to_smem(cbar, Fs, CM->Ftile[s] + size_t(tile_idx) * Js * EP, static_cast<uint32_t>(sizeof(double) * Js * EP));
+      chrom_coefficients<RB, INJECT, EPK_THREADS>(P, *CM, K, s, zoff, zld, psr, r0, nr, rgroup0, Asx, tid);
+      __syncthreads();
+      mbar_wait(cbar, phase);
+      phase ^= 1;
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int l = 0; l < 2; ++l) acc[i][l][0] = acc[i][l][1] = acc[i][l][2] = 0.0;
+      if (e0 < tile.n_ep) epk_gemm(Fs, Asx, Js, (Js * ks) / nsplit, (Js * (ks + 1)) / nsplit, e0, rp, nd, acc);
+      if (nsplit > 1) epk_split_k(Fs, ks, nsplit, gthreads, tg, acc);
+      if (ks == 0 && chunk < n_chunks) {
+        const int rl = (2 * rp) & 15;
+        double* blockp = P.Cbuf + (size_t(tile.reserved) * n_chunks + size_t(chunk) * tile.n_ep) * css_u;
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const int e = e0 + i;
+          if (e < tile.n_ep) {
+            double2* o = reinterpret_cast<double2*>(blockp + size_t(e) * css_u + 48 * (1 + s) + rl * 3);
+            __stcg(o, make_double2(acc[i][0][0], acc[i][0][1]));
+            __stcg(o + 1, make_double2(acc[i][0][2], acc[i][1][0]));
+            __stcg(o + 2, make_double2(acc[i][1][1], acc[i][1][2]));
+          }
+        }
+      }
+    }
+  }
+}
+
+template <bool INJECT>
+__global__ void __launch_bounds__(EPK_THREADS, 2) epoch_kernel(const ptar_gen_params P, const PhiloxKeys K) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  epoch_body<INJECT, 0>(P, K, smem_raw, nullptr);
+}
+
+template <bool INJECT>
+__global__ void __launch_bounds__(EPK_THREADS, 2) epoch_chrom_kernel(const ptar_gen_params P, const PhiloxKeys K,
+                                                                     const ptar_chrom_model CM) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  epoch_body<INJECT, 1>(P, K, smem_raw, &CM);
 }
 
 }  // namespace ptar

@@ -34,15 +34,22 @@ def pulsar_names(noise_params: dict, require_red: bool = True) -> list:
 
 
 def per_pulsar(noise_params: dict, name: str) -> dict:
-    """``{'backends': [...], 'efac': arr, 'log10_equad': arr, 'log10_ecorr': arr, 'rn_log10_A', 'rn_gamma'}``."""
+    """``{'backends': [...], 'efac': arr, 'log10_equad': arr, 'log10_ecorr': arr, 'rn_log10_A', 'rn_gamma', 'dm_log10_A',
+    'dm_gamma', 'chrom_log10_A', 'chrom_gamma', 'chrom_idx'}``; each process's values are None when its keys are absent."""
     pre = name + "_"
     be = {}
     out = {"rn_log10_A": None, "rn_gamma": None}
+    # chromatic processes (enterprise_extensions' dm_gp / chrom_gp names); chrom_idx defaults to 4 when absent
+    chrom = {"dm_gp_log10_A": "dm_log10_A", "dm_gp_gamma": "dm_gamma", "chrom_gp_log10_A": "chrom_log10_A",
+             "chrom_gp_gamma": "chrom_gamma", "chrom_gp_idx": "chrom_idx"}
+    out.update({v: None for v in chrom.values()})
     for k, v in noise_params.items():
         if not k.startswith(pre):
             continue
         rest = k[len(pre):]
-        if rest == "red_noise_gamma":
+        if rest in chrom:
+            out[chrom[rest]] = v
+        elif rest == "red_noise_gamma":
             out["rn_gamma"] = v
         elif rest == "red_noise_log10_A":
             out["rn_log10_A"] = v
@@ -59,4 +66,6 @@ def per_pulsar(noise_params: dict, name: str) -> dict:
     out["efac"] = np.array([be[b].get("efac", 1.0) for b in names])
     out["log10_equad"] = np.array([be[b].get("equad", -300.0) for b in names])
     out["log10_ecorr"] = np.array([be[b].get("ecorr", -300.0) for b in names])
+    if out["chrom_log10_A"] is not None and out["chrom_idx"] is None:
+        out["chrom_idx"] = 4.0
     return out

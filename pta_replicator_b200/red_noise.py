@@ -86,6 +86,37 @@ def add_red_noise(psr: SimulatedPulsar, log10_amplitude: float, spectral_index: 
     psr.update_residuals()
 
 
+def _add_chromatic(psr, slot, suffix, log10_amplitude, spectral_index, idx, components, seed, fref):
+    """One chromatic slot of a one-pulsar exact-epochs batch, injected with ``np.random.randn(2 components)``."""
+    if seed is not None:
+        np.random.seed(seed)
+    batch = PulsarBatch([psr], exact_epochs=True)
+    batch._set_chrom(slot, 0, log10_amplitude, spectral_index, idx, components, None, fref)
+    z = np.random.randn(2 * components)
+    torch = batch.torch
+    row = batch.generate(1, inject=dict(zchr=torch.from_numpy(z)[None, None, :]))[0]
+    dt = TimeArray(batch.unpack(row, 0), "s")
+    psr.update_added_signals("{}_{}".format(psr.name, suffix),
+                             {"amplitude": log10_amplitude, "spectral_index": spectral_index, "idx": idx, "fref": fref}, dt)
+    psr.toas.adjust_TOAs(dt.to("day"))
+    psr.update_residuals()
+
+
+def add_dm_noise(psr: SimulatedPulsar, log10_amplitude: float, spectral_index: float, components: int = 30,
+                 seed: int = None, fref: float = 1400.0):
+    """Dispersion-measure variations (extension; the reference has no chromatic noise): the power-law Gaussian process of
+    ``add_red_noise`` on the basis (fref / nu)^2 (sin, cos)(2 pi k t / T), enterprise's ``createfourierdesignmatrix_dm``
+    with the ``powerlaw`` prior.  Draws ``np.random.randn(2 components)``."""
+    _add_chromatic(psr, 0, "dm_gp", log10_amplitude, spectral_index, 2.0, components, seed, fref)
+
+
+def add_chromatic_noise(psr: SimulatedPulsar, log10_amplitude: float, spectral_index: float, idx: float = 4.0,
+                        components: int = 30, seed: int = None, fref: float = 1400.0):
+    """A chromatic Gaussian process (extension; scattering for ``idx`` = 4): as ``add_dm_noise`` with the weight
+    (fref / nu)^idx, enterprise's ``createfourierdesignmatrix_chromatic``."""
+    _add_chromatic(psr, 1, "chrom_gp", log10_amplitude, spectral_index, idx, components, seed, fref)
+
+
 def add_gwb(psrs: list, log10_amplitude: float, spectral_index: float, no_correlations: bool = False,
             seed: int = None, turnover: bool = False, clm: list = [np.sqrt(4.0 * np.pi)], lmax: int = 0,
             f0: float = 1e-9, beta: float = 1, power: float = 1, userSpec: np.ndarray = None, npts: int = 600,

@@ -83,7 +83,7 @@ class TOAs:
         self.site = list(site) if site is not None else ["AXIS"] * n
         self.names = list(names) if names is not None else ["fake"] * n
         fl = _FlagColumn(dict(f) for f in flags) if flags is not None else _FlagColumn({} for _ in range(n))
-        self.table = {"tdbld": mjd.copy(), "mjd_float": np.asarray(mjd, dtype=float), "flags": fl}
+        self.table = {"tdbld": mjd.copy(), "mjd_float": np.asarray(mjd, dtype=float), "flags": fl, "freq": self.freq}
         self.delay_s = np.zeros(n)  # accumulated injected delay [s]
 
     def __len__(self):

@@ -59,3 +59,23 @@ def ng15_recipe(batch, noise, gw_log10_A=-14.6733, gw_gamma=13.0 / 3.0, componen
     if gwb:
         batch.set_gwb(gw_log10_A, gw_gamma)
     return batch
+
+
+# receiver bands [MHz] by a substring of the backend name; anything else observes at L band
+RECEIVER_BANDS = (("430", (422.0, 442.0)), ("Rcvr_800", (720.0, 920.0)), ("L-wide", (1150.0, 1880.0)),
+                  ("Rcvr1_2", (1150.0, 1880.0)), ("S-wide", (1700.0, 2400.0)))
+
+
+def spread_subband_frequencies(psrs):
+    """Give every epoch's sub-band TOAs (runs < 10 s apart) radio frequencies spread evenly over the band of the epoch's
+    backend (flag ``f``), in place, so that chromatic processes see a realistic frequency coverage."""
+    for p in psrs:
+        t = np.asarray(p.toas.table["tdbld"], dtype=np.float64) * 86400.0
+        fl = p.toas.table["flags"]
+        o = np.argsort(t, kind="stable")
+        starts = np.flatnonzero(np.r_[True, np.diff(t[o]) > 10.0])
+        for a, z in zip(starts, np.r_[starts[1:], len(o)]):
+            be = str(fl[int(o[a])].get("f"))
+            lo, hi = next((b for key, b in RECEIVER_BANDS if key in be), (1150.0, 1880.0))
+            p.toas.freq[o[a:z]] = np.linspace(lo, hi, z - a) if z - a > 1 else 0.5 * (lo + hi)
+    return psrs
