@@ -62,6 +62,8 @@
  *   ptar_fs_y2 /           no counterpart (a refit of a spectral model to the free spectrum per realization, as
  *   ptar_fs_refit          ceffyl does from KDEs): power-law, turnover or user spectra on a grid, exact in the factorised
  *                          per-bin likelihoods, reduced by ptar_curn_reduce
+ *   ptar_cw_population     add_cgw per realization with parameters drawn from priors on the device (a population study
+ *                          calls add_cgw once per realization)                   deterministic.py:13-163
  *   ptar_bwm_sky /         no counterpart (a matched-filter search of add_gw_memory's ramp per realization): the
  *   ptar_bwm_combine       coherent burst-with-memory statistic over epoch x sky and the pulsar-term statistic, reduced
  *                          on the device
@@ -95,7 +97,9 @@ extern "C" {
                              PTAR_BURST_MAX_TEMPLATE / _GROUP / _TB) and the free spectrum's spectral refit
                              (ptar_fs_refit_model, ptar_fs_y2, ptar_fs_refit, PTAR_FS_MAX_TEMPLATE) and chromatic noise in
                              the generator (ptar_chrom_model, ptar_generate_chrom, ptar_generate_stage_chrom,
-                             ptar_run_job_to_host_chrom, PTAR_K_CHROM, PTAR_CHROM_SLOTS) are new symbols only, so
+                             ptar_run_job_to_host_chrom, PTAR_K_CHROM, PTAR_CHROM_SLOTS) and per-realization
+                             continuous-wave populations (ptar_cwpop_model, ptar_cw_population[_stage], PTAR_K_CWPOP,
+                             PTAR_CWPOP_*) are new symbols only, so
                              a caller detects them by looking the symbol up.  ptar_os_project accepts nc up to
                              PTAR_RN_MAX_NC since the red-noise likelihood; nothing changes for nc <= PTAR_OS_MAX_NC. */
 
@@ -120,6 +124,7 @@ extern "C" {
 #define PTAR_K_RED    4
 #define PTAR_K_GWB    5
 #define PTAR_K_CHROM  6   /* chromatic coefficients: index = (slot << 16) | Fourier column */
+#define PTAR_K_CWPOP  7   /* continuous-wave populations: index = source * 16 + parameter pair, see ptar_cw_population */
 
 /* One tile of the packed TOA axis: <=1024 consecutive (time-sorted) TOAs of ONE pulsar
  * touching <=64 kernel-epochs. */
@@ -828,6 +833,62 @@ typedef struct {
 
 int ptar_fs_y2(const double* X, int32_t nreal, const ptar_fs_model* fm, double* y2, void* stream);
 int ptar_fs_refit(const double* y2, int32_t nreal, const ptar_fs_refit_model* rm, double* lnL, void* stream);
+
+/* Per-realization continuous-wave populations (csrc/ptar_cwpop.cuh).  Every realization r of [real0, real0 + nreal)
+ * gets n_src sources; each source parameter j is fixed (kind PTAR_CWPOP_FIXED: lo), uniform (PTAR_CWPOP_UNIFORM:
+ * lo + width u) or isotropic (PTAR_CWPOP_ACOS: acos(lo + width u), lo = -1, width = 2), the affine map rounded operation
+ * by operation.  The uniforms u are 53-bit, (a >> 5) 2^26 + (b >> 6) times 2^-53, from the Philox4x32-10 words
+ * (a, b) = (w.x, w.y) and (w.z, w.w) of the counter (source * 16 + j / 2, PTAR_K_CWPOP, r & 0xffffffff, r >> 32):
+ * parameter j takes the first word pair for even j and the second for odd j.  With pphase the pulsar-term phase of pulsar
+ * p is 2 pi u, u the first pair of (source * 16 + 4, PTAR_K_CWPOP | p << 8, r).  Parameters are drawn whether or not
+ * they are used, so a draw does not depend on the others' kinds; the noise streams (kinds 1-6) are untouched.
+ * From the draws: h0, fgw and Mc are 10^(log10 value); d_L = 2 Mc^(5/3) (pi fgw)^(2/3) / h0 (geometric units), and the
+ * source is then add_cgw's (deterministic.py:13-163) with pdist [kpc] or the drawn pulsar phase, mode 0 (evolve),
+ * 1 (phase_approx) or 2 (monochromatic) and psr_term.  A source whose 1 + Omega.p is below PTAR_CWPOP_POLE_TOL
+ * (or NaN) at pulsar p has antenna pattern (0, 0) there; a NaN contribution (a merged binary) is dropped.
+ *   stage 1 (draw)  scratch <- per-(r, s) source scalars [nreal][n_src][16] and per-(r, s, p) pulsar constants
+ *                   [nreal][n_src][n_psr][8]; params (optional) <- [nreal][n_src][PTAR_CWPOP_TABLE] = {gwtheta, gwphi,
+ *                   phase0, psi, inc, log10_h0, log10_fgw, log10_mc, dist [Mpc], fgw, Mc, h0, 0, 0, 0, 0}, followed with
+ *                   pphase by [nreal][n_src][n_psr] pulsar phases.
+ *   stage 2 (add)   rows[r][i] += sum_s delay of source s at slot i for every slot with slot_psr[i] >= 0.
+ * ptar_cw_population runs both (stage 0 of ptar_cw_population_stage); with rows == NULL it only draws.
+ * scratch_len >= nreal * n_src * (16 + 8 n_psr).  Outputs are bit-identical whatever nreal, chunking or real0. */
+#define PTAR_CWPOP_MAX_SRC 64    /* sources per realization                                               */
+#define PTAR_CWPOP_NPAR    8     /* drawn parameters per source                                           */
+#define PTAR_CWPOP_TABLE   16    /* doubles per (r, s) row of the parameter table                          */
+#define PTAR_CWPOP_POLE_TOL 1e-12
+#define PTAR_CWPOP_FIXED   0
+#define PTAR_CWPOP_UNIFORM 1
+#define PTAR_CWPOP_ACOS    2
+#define PTAR_CWPOP_LOG10_H0  0   /* parameter indices: the order of the counter's parameter pairs          */
+#define PTAR_CWPOP_LOG10_FGW 1
+#define PTAR_CWPOP_LOG10_MC  2
+#define PTAR_CWPOP_GWTHETA   3
+#define PTAR_CWPOP_GWPHI     4
+#define PTAR_CWPOP_PHASE0    5
+#define PTAR_CWPOP_PSI       6
+#define PTAR_CWPOP_INC       7
+typedef struct {
+  int32_t n_psr;                       /* >= 1                                                                 */
+  int32_t n_src;                       /* 1 .. PTAR_CWPOP_MAX_SRC                                              */
+  int32_t mode;                        /* 0 evolve, 1 phase_approx, 2 monochromatic                            */
+  int32_t psr_term;                    /* 1: Earth and pulsar terms, 0: Earth term only                        */
+  int32_t pphase;                      /* 1: pulsar-term phase drawn per (r, s, p), pd from it; 0: pd = pdist  */
+  int32_t kind[PTAR_CWPOP_NPAR];       /* PTAR_CWPOP_FIXED / _UNIFORM / _ACOS                                  */
+  int32_t reserved;
+  double lo[PTAR_CWPOP_NPAR];
+  double width[PTAR_CWPOP_NPAR];
+  const double* phat;                  /* [n_psr][3] pulsar unit vectors                                       */
+  const double* pdist;                 /* [n_psr] pulsar distances [kpc] (may be NULL with pphase)             */
+  const double* slot_t;                /* [ld] TOA (MJD 86400) - tref [s] per slot of the packed axis          */
+  const int32_t* slot_psr;             /* [ld] pulsar of each slot, -1 for alignment slots (never written)     */
+} ptar_cwpop_model;
+
+int ptar_cw_population(double* rows, int64_t ld, int32_t nreal, int64_t real0, uint64_t seed, const ptar_cwpop_model* m,
+                       double* scratch, int64_t scratch_len, double* params, void* stream);
+int ptar_cw_population_stage(double* rows, int64_t ld, int32_t nreal, int64_t real0, uint64_t seed,
+                             const ptar_cwpop_model* m, double* scratch, int64_t scratch_len, double* params, int stage,
+                             void* stream);
 
 /* End-to-end job: GWB mix + synth + generate for realizations [real0, real0+nreal), then
  * (ptar_run_job_to_host) copy the residuals to pinned host memory, chunk by chunk, with the

@@ -53,7 +53,7 @@ def max_red_columns(rc=16, split_epoch=False):
 
 F_WHITE, F_ECORR, F_RED, F_GWB, F_DET, F_WHITE1 = 1, 2, 4, 8, 16, 32
 TM_KMAX = 32                                       # timing-model columns per pulsar (PTAR_TM_KMAX)
-K_WHITE1, K_WHITE2, K_ECORR, K_RED, K_GWB, K_CHROM = 1, 2, 3, 4, 5, 6
+K_WHITE1, K_WHITE2, K_ECORR, K_RED, K_GWB, K_CHROM, K_CWPOP = 1, 2, 3, 4, 5, 6, 7
 CHROM_SLOTS = 2                                    # chromatic slots of ptar_generate_chrom (PTAR_CHROM_SLOTS)
 
 EXPORTS = ("ptar_version", "ptar_last_error", "ptar_cholesky_lower", "ptar_fourier_basis", "ptar_cgw_delay", "ptar_cw_catalog", "ptar_burst_delay", "ptar_memory_delay",
@@ -64,7 +64,8 @@ EXPORTS = ("ptar_version", "ptar_last_error", "ptar_cholesky_lower", "ptar_fouri
            "ptar_fp_reduce_fap", "ptar_fe_sky", "ptar_fe_combine", "ptar_curn_grid", "ptar_curn_reduce",
            "ptar_hd_grid", "ptar_rn_grid", "ptar_bwm_sky", "ptar_bwm_combine", "ptar_fs_grid",
            "ptar_burst_ninv", "ptar_burst_project", "ptar_burst_reduce", "ptar_fs_y2", "ptar_fs_refit",
-           "ptar_generate_chrom", "ptar_generate_stage_chrom", "ptar_run_job_to_host_chrom")
+           "ptar_generate_chrom", "ptar_generate_stage_chrom", "ptar_run_job_to_host_chrom",
+           "ptar_cw_population", "ptar_cw_population_stage")
 OS_MAX_NC, OS_MAX_ORF, OS_MAX_PSR = 32, 4, 256     # optimal statistic: GW-basis columns, templates, pulsars (ptar.h)
 OS_MAX_NULL = 65536                                # null columns of ptar_os_null (PTAR_OS_MAX_NULL)
 OS_NULL_PHASE_SHIFT, OS_NULL_SKY_SCRAMBLE = 1, 2
@@ -80,6 +81,9 @@ BWM_MAX_EPOCH = 512                                # burst-with-memory search: b
 FS_MAX_PSR, FS_MAX_BIN, FS_JB = 256, 32, 32       # free-spectrum likelihood: pulsars, bins, eigen-rows per block (ptar.h)
 FS_MAX_TEMPLATE = 65536                            # spectral refit: templates of one model (PTAR_FS_MAX_TEMPLATE)
 BURST_MAX_TEMPLATE, BURST_GROUP, BURST_TB = 4096, 256, 16   # burst search: templates, per group, per CTA (ptar.h)
+CWPOP_MAX_SRC, CWPOP_NPAR, CWPOP_TABLE = 64, 8, 16  # CW populations: sources per realization, drawn parameters, table row
+CWPOP_SRC, CWPOP_PSR = 16, 8                       # doubles per (r, s) and per (r, s, p) record of the scratch (ptar_cwpop.cuh)
+CWPOP_FIXED, CWPOP_UNIFORM, CWPOP_ACOS = 0, 1, 2   # parameter kinds of ptar_cwpop_model
 BWM_LINV = 6                                       # packed L2^-1 doubles per (epoch pair, sky point) (csrc/ptar_bwm.cuh)
 
 
@@ -203,6 +207,13 @@ class FsRefitModel(C.Structure):
                 ("lam", C.c_void_p), ("rho2", C.c_void_p), ("ldet", C.c_void_p)]
 
 
+class CwPopModel(C.Structure):
+    _fields_ = [("n_psr", C.c_int32), ("n_src", C.c_int32), ("mode", C.c_int32), ("psr_term", C.c_int32),
+                ("pphase", C.c_int32), ("kind", C.c_int32 * CWPOP_NPAR), ("reserved", C.c_int32),
+                ("lo", C.c_double * CWPOP_NPAR), ("width", C.c_double * CWPOP_NPAR), ("phat", C.c_void_p),
+                ("pdist", C.c_void_p), ("slot_t", C.c_void_p), ("slot_psr", C.c_void_p)]
+
+
 _lib = None
 
 
@@ -276,6 +287,8 @@ def lib():
     L.ptar_generate_stage_chrom.argtypes = [C.POINTER(GenParams), C.POINTER(ChromModel), i32, vp]
     L.ptar_run_job_to_host_chrom.argtypes = [C.POINTER(Job), vp, C.POINTER(ChromModel), vp, i64, i64, i64, C.c_int32, vp, vp,
                                              vp, vp, vp]
+    L.ptar_cw_population.argtypes = [vp, i64, C.c_int32, i64, u64, vp, vp, i64, vp, vp]   # m: address of a CwPopModel
+    L.ptar_cw_population_stage.argtypes = [vp, i64, C.c_int32, i64, u64, vp, vp, i64, vp, i32, vp]
     for name in EXPORTS:
         if name not in ("ptar_version", "ptar_last_error"):
             getattr(L, name).restype = C.c_int

@@ -12,6 +12,7 @@
 #include "ptar_burst.cuh"
 #include "ptar_bwm.cuh"
 #include "ptar_curn.cuh"
+#include "ptar_cwpop.cuh"
 #include "ptar_generate.cuh"
 #include "ptar_gwb.cuh"
 #include "ptar_gwb_i8.cuh"
@@ -1335,6 +1336,49 @@ int ptar_fs_refit(const double* y2, int32_t nreal, const ptar_fs_refit_model* rm
   if (int rc = opt_in_smem(ptar::fs_refit_kernel, optin, ptar::RF_SMEM, "ptar_fs_refit")) return rc;
   ptar::fs_refit_kernel<<<grid, ptar::RF_THREADS, ptar::RF_SMEM, static_cast<cudaStream_t>(stream)>>>(y2, nreal, *rm, lnL);
   return check_launch("ptar_fs_refit");
+}
+
+int ptar_cw_population_stage(double* rows, int64_t ld, int32_t nreal, int64_t real0, uint64_t seed, const ptar_cwpop_model* m,
+                             double* scratch, int64_t scratch_len, double* params, int stage, void* stream) {
+  if (!m || !scratch || nreal <= 0 || real0 < 0 || stage < 0 || stage > 2) return fail(-1, "ptar_cw_population: bad argument%s");
+  if (m->n_psr <= 0 || m->n_src < 1 || m->n_src > PTAR_CWPOP_MAX_SRC || m->mode < 0 || m->mode > 2 || !m->phat)
+    return fail(-2, "ptar_cw_population: need n_psr >= 1, 1 <= n_src <= 64, mode 0..2 and phat%s");
+  if (!m->pphase && !m->pdist) return fail(-2, "ptar_cw_population: pdist missing (no drawn pulsar phase)%s");
+  for (int j = 0; j < PTAR_CWPOP_NPAR; ++j)
+    if (m->kind[j] < PTAR_CWPOP_FIXED || m->kind[j] > PTAR_CWPOP_ACOS) return fail(-2, "ptar_cw_population: bad parameter kind%s");
+  const int64_t pairs = int64_t(nreal) * m->n_src;
+  if (scratch_len < pairs * (ptar::CWP_SRC + int64_t(ptar::CWP_PSR) * m->n_psr))
+    return fail(-2, "ptar_cw_population: scratch too small (need nreal * n_src * (16 + 8 n_psr) doubles)%s");
+  if (rows && (ld <= 0 || !m->slot_t || !m->slot_psr)) return fail(-2, "ptar_cw_population: rows need ld, slot_t and slot_psr%s");
+  if (!rows && stage == 2) return fail(-2, "ptar_cw_population: the add stage needs rows%s");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  double* src = scratch;
+  double* psr = scratch + pairs * ptar::CWP_SRC;
+  if (stage != 2) {
+    double* pph = params && m->pphase ? params + pairs * PTAR_CWPOP_TABLE : nullptr;
+    ptar::cwpop_draw_kernel<<<static_cast<unsigned>((pairs + 127) / 128), 128, 0, st>>>(src, psr, params, pph, *m, nreal,
+                                                                                        real0, seed);
+    if (int rc = check_launch("ptar_cw_population (draw)")) return rc;
+  }
+  if (!rows || stage == 1) return 0;
+  const int64_t rb = (nreal + ptar::CWP_RB - 1) / ptar::CWP_RB;
+  if (rb > 65535) return fail(-3, "ptar_cw_population: too many realizations per call%s");
+  const dim3 grid(static_cast<unsigned>((ld + ptar::CWP_TOAS - 1) / ptar::CWP_TOAS), static_cast<unsigned>(rb));
+  if (m->mode == 0)
+    ptar::cwpop_add_kernel<0><<<grid, ptar::CWP_TOAS, 0, st>>>(rows, ld, nreal, src, psr, m->slot_t, m->slot_psr, m->n_psr,
+                                                               m->n_src, m->psr_term);
+  else if (m->mode == 1)
+    ptar::cwpop_add_kernel<1><<<grid, ptar::CWP_TOAS, 0, st>>>(rows, ld, nreal, src, psr, m->slot_t, m->slot_psr, m->n_psr,
+                                                               m->n_src, m->psr_term);
+  else
+    ptar::cwpop_add_kernel<2><<<grid, ptar::CWP_TOAS, 0, st>>>(rows, ld, nreal, src, psr, m->slot_t, m->slot_psr, m->n_psr,
+                                                               m->n_src, m->psr_term);
+  return check_launch("ptar_cw_population (add)");
+}
+
+int ptar_cw_population(double* rows, int64_t ld, int32_t nreal, int64_t real0, uint64_t seed, const ptar_cwpop_model* m,
+                       double* scratch, int64_t scratch_len, double* params, void* stream) {
+  return ptar_cw_population_stage(rows, ld, nreal, real0, seed, m, scratch, scratch_len, params, 0, stream);
 }
 
 }  // extern "C"

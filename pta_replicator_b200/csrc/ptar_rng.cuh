@@ -79,6 +79,10 @@ __device__ __forceinline__ void box_muller(uint32_t a, uint32_t b, float& n0, fl
 // Counter layout: c.x = element index (TOA within the pulsar / ECORR bucket / Fourier column /
 // grid column), c.y = kind | psr << 8, (c.z, c.w) = global realization id >> 2.  The 4 outputs
 // of a counter are the realizations id&~3 .. +3 of that element.
+// The continuous-wave population stream (kind 7, ptar_cwpop.cuh) is keyed per realization instead: c.x = source * 16 +
+// parameter pair (4 = the pulsar-term phase), c.y = 7 | psr << 8 (psr only for that phase), (c.z, c.w) = the full global
+// realization id; its 4 words are two 53-bit uniforms, (w.x >> 5) 2^26 + (w.y >> 6) and (w.z >> 5) 2^26 + (w.w >> 6)
+// times 2^-53.
 __device__ __forceinline__ void normals4(float n[4], uint32_t block, uint32_t kind, uint32_t psr,
                                          uint64_t rfield, const PhiloxKeys& K) {
   const uint4 w = philox4x32_10(make_uint4(block, kind | (psr << 8), static_cast<uint32_t>(rfield),
