@@ -64,6 +64,9 @@
  *                          per-bin likelihoods, reduced by ptar_curn_reduce
  *   ptar_cw_population     add_cgw per realization with parameters drawn from priors on the device (a population study
  *                          calls add_cgw once per realization)                   deterministic.py:13-163
+ *   ptar_common_population no counterpart (a calibration study draws a common process per realization on the host): a
+ *                          power-law or free-spectrum common process, uncorrelated or ORF-correlated, drawn from priors
+ *                          on the device in the statistics' Fourier basis and added to every realization
  *   ptar_bwm_sky /         no counterpart (a matched-filter search of add_gw_memory's ramp per realization): the
  *   ptar_bwm_combine       coherent burst-with-memory statistic over epoch x sky and the pulsar-term statistic, reduced
  *                          on the device
@@ -99,7 +102,8 @@ extern "C" {
                              the generator (ptar_chrom_model, ptar_generate_chrom, ptar_generate_stage_chrom,
                              ptar_run_job_to_host_chrom, PTAR_K_CHROM, PTAR_CHROM_SLOTS) and per-realization
                              continuous-wave populations (ptar_cwpop_model, ptar_cw_population[_stage], PTAR_K_CWPOP,
-                             PTAR_CWPOP_*) are new symbols only, so
+                             PTAR_CWPOP_*) and per-realization common-process populations (ptar_cpop_model,
+                             ptar_common_population[_stage], PTAR_K_CPOP, PTAR_CPOP_*) are new symbols only, so
                              a caller detects them by looking the symbol up.  ptar_os_project accepts nc up to
                              PTAR_RN_MAX_NC since the red-noise likelihood; nothing changes for nc <= PTAR_OS_MAX_NC. */
 
@@ -125,6 +129,7 @@ extern "C" {
 #define PTAR_K_GWB    5
 #define PTAR_K_CHROM  6   /* chromatic coefficients: index = (slot << 16) | Fourier column */
 #define PTAR_K_CWPOP  7   /* continuous-wave populations: index = source * 16 + parameter pair, see ptar_cw_population */
+#define PTAR_K_CPOP   8   /* common-process populations: index = bin or PTAR_CPOP_HYPER + pair, see ptar_common_population */
 
 /* One tile of the packed TOA axis: <=1024 consecutive (time-sorted) TOAs of ONE pulsar
  * touching <=64 kernel-epochs. */
@@ -889,6 +894,56 @@ int ptar_cw_population(double* rows, int64_t ld, int32_t nreal, int64_t real0, u
 int ptar_cw_population_stage(double* rows, int64_t ld, int32_t nreal, int64_t real0, uint64_t seed,
                              const ptar_cwpop_model* m, double* scratch, int64_t scratch_len, double* params, int stage,
                              void* stream);
+
+/* Per-realization common-process populations (csrc/ptar_cpop.cuh).  Every realization r of [real0, real0 + nreal)
+ * gets the Fourier coefficients c[r][a][2k + s] = sqrt(phi_k(r)) sum_b B_ab z[r][b][2k + s] of a common process on the
+ * basis F_a = (sin, cos)(2 pi f_k t) (s = 0, 1), f_k = freqs[k], k < K, and rows[r][i] += sum_j c[r][p(i)][j] F_j(t_i).
+ * Hyperparameters: uniforms u through cwpop_param's affine map (kind PTAR_CWPOP_FIXED: lo, PTAR_CWPOP_UNIFORM:
+ * lo + width u, each operation rounded once).  The power law (PTAR_CPOP_POWERLAW) draws h = (log10_A, gamma) and has
+ * phi_k = A^2 phi~_k, A = 10^log10_A, phi~_k = (pl_x[k]^-gamma / pl_den) pl_y3 (engine._powerlaw_prior's operations:
+ * pl_x[k] = f_k yr, pl_den = 12 pi^2 Tspan, pl_y3 = yr^3); the free spectrum (PTAR_CPOP_FREE) draws h = log10_rho_k
+ * per bin (kind[0], lo[0], width[0] for every bin) and has sqrt(phi_k) = 10^log10_rho_k.
+ * Counters of Philox4x32-10, (c.z, c.w) = the full global realization id:
+ *   hyperparameter pair j / 2:  (PTAR_CPOP_HYPER + j / 2, PTAR_K_CPOP, r); h_j takes the word pair (w.x, w.y) for even
+ *                               j and (w.z, w.w) for odd j, each a 53-bit uniform (a >> 5) 2^26 + (b >> 6) times 2^-53;
+ *   normals of pulsar b, bin k: (k, PTAR_K_CPOP | b << 8, r); u1, u2 the two 53-bit uniforms, rho = sqrt(-2 ln(1 - u1)),
+ *                               theta = 2 pi u2: z[r][b][2k] = rho cos theta, z[r][b][2k + 1] = rho sin theta (fp64).
+ * The noise streams (kinds 1-7) are untouched, so every realization's noise is what it is without a population, and
+ * the draws do not depend on nreal, chunking or real0.  B (Bt = B^T, row-major [n_psr][n_psr]) is the ORF factor,
+ * Gamma = B B^T; Bt == NULL is Gamma = I (uncorrelated).  The mixing sums over b in index order, unfused.
+ *   stage 1 (draw)  scratch <- c [nreal][n_psr][2K]; params (optional) <- [nreal][2] (log10_A, gamma) or [nreal][K]
+ *                   (log10_rho_k).
+ *   stage 2 (add)   rows[r][i] += sum_j c[r][slot_psr[i]][j] F_j(slot_t[i]) for every slot with slot_psr[i] >= 0,
+ *                   the argument rounded as (2 pi t) f_k; alignment slots are never touched.
+ * ptar_common_population runs both (stage 0 of ptar_common_population_stage); with rows == NULL it only draws.
+ * scratch_len >= nreal * n_psr * 2K.  Outputs are bit-identical whatever nreal, chunking or real0. */
+#define PTAR_CPOP_MAX_K    32         /* Fourier bins                                                          */
+#define PTAR_CPOP_MAX_PSR  2048       /* pulsars (the draw kernel holds one bin's 2 n_psr normals in shared)   */
+#define PTAR_CPOP_HYPER    0x10000    /* first counter element of the hyperparameter pairs                     */
+#define PTAR_CPOP_POWERLAW 0
+#define PTAR_CPOP_FREE     1
+typedef struct {
+  int32_t n_psr;                       /* 1 .. PTAR_CPOP_MAX_PSR                                               */
+  int32_t K;                           /* 1 .. PTAR_CPOP_MAX_K                                                 */
+  int32_t spectrum;                    /* PTAR_CPOP_POWERLAW / PTAR_CPOP_FREE                                  */
+  int32_t kind[2];                     /* PTAR_CWPOP_FIXED / _UNIFORM of (log10_A, gamma); free: kind[0]       */
+  int32_t reserved;
+  double lo[2];
+  double width[2];
+  double pl_den;                       /* 12 pi^2 Tspan (power law)                                            */
+  double pl_y3;                        /* yr^3 [s^3] (power law)                                               */
+  const double* pl_x;                  /* [K] f_k yr (power law)                                               */
+  const double* freqs;                 /* [K] f_k [Hz]                                                         */
+  const double* Bt;                    /* [n_psr][n_psr] B^T of Gamma = B B^T, or NULL (Gamma = I)             */
+  const double* slot_t;                /* [ld] absolute TDB time [s] per slot of the packed axis               */
+  const int32_t* slot_psr;             /* [ld] pulsar of each slot, -1 for alignment slots (never written)     */
+} ptar_cpop_model;
+
+int ptar_common_population(double* rows, int64_t ld, int32_t nreal, int64_t real0, uint64_t seed,
+                           const ptar_cpop_model* m, double* scratch, int64_t scratch_len, double* params, void* stream);
+int ptar_common_population_stage(double* rows, int64_t ld, int32_t nreal, int64_t real0, uint64_t seed,
+                                 const ptar_cpop_model* m, double* scratch, int64_t scratch_len, double* params,
+                                 int stage, void* stream);
 
 /* End-to-end job: GWB mix + synth + generate for realizations [real0, real0+nreal), then
  * (ptar_run_job_to_host) copy the residuals to pinned host memory, chunk by chunk, with the

@@ -11,6 +11,7 @@
 #include "../../include/ptar.h"
 #include "ptar_burst.cuh"
 #include "ptar_bwm.cuh"
+#include "ptar_cpop.cuh"
 #include "ptar_curn.cuh"
 #include "ptar_cwpop.cuh"
 #include "ptar_generate.cuh"
@@ -1379,6 +1380,49 @@ int ptar_cw_population_stage(double* rows, int64_t ld, int32_t nreal, int64_t re
 int ptar_cw_population(double* rows, int64_t ld, int32_t nreal, int64_t real0, uint64_t seed, const ptar_cwpop_model* m,
                        double* scratch, int64_t scratch_len, double* params, void* stream) {
   return ptar_cw_population_stage(rows, ld, nreal, real0, seed, m, scratch, scratch_len, params, 0, stream);
+}
+
+int ptar_common_population_stage(double* rows, int64_t ld, int32_t nreal, int64_t real0, uint64_t seed,
+                                 const ptar_cpop_model* m, double* scratch, int64_t scratch_len, double* params, int stage,
+                                 void* stream) {
+  if (!m || !scratch || nreal <= 0 || real0 < 0 || stage < 0 || stage > 2) return fail(-1, "ptar_common_population: bad argument%s");
+  if (m->n_psr < 1 || m->n_psr > PTAR_CPOP_MAX_PSR || m->K < 1 || m->K > PTAR_CPOP_MAX_K || !m->freqs)
+    return fail(-2, "ptar_common_population: need 1 <= n_psr <= 2048, 1 <= K <= 32 and freqs%s");
+  if (m->spectrum != PTAR_CPOP_POWERLAW && m->spectrum != PTAR_CPOP_FREE) return fail(-2, "ptar_common_population: bad spectrum%s");
+  if (m->spectrum == PTAR_CPOP_POWERLAW && !m->pl_x) return fail(-2, "ptar_common_population: the power law needs pl_x%s");
+  for (int j = 0; j < 2; ++j)
+    if (m->kind[j] != PTAR_CWPOP_FIXED && m->kind[j] != PTAR_CWPOP_UNIFORM) return fail(-2, "ptar_common_population: bad parameter kind%s");
+  const int64_t per_real = int64_t(m->n_psr) * 2 * m->K;
+  if (scratch_len < nreal * per_real) return fail(-2, "ptar_common_population: scratch too small (need nreal * n_psr * 2K doubles)%s");
+  if (rows && (ld <= 0 || !m->slot_t || !m->slot_psr)) return fail(-2, "ptar_common_population: rows need ld, slot_t and slot_psr%s");
+  if (!rows && stage == 2) return fail(-2, "ptar_common_population: the add stage needs rows%s");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (stage != 2) {
+    const int64_t ctas = int64_t(nreal) * m->K;
+    if (ctas > INT32_MAX) return fail(-3, "ptar_common_population: too many realizations per call%s");
+    ptar::cpop_draw_kernel<<<static_cast<unsigned>(ctas), ptar::CPOP_DRAW_THREADS, 2 * m->n_psr * sizeof(double), st>>>(
+        scratch, params, *m, real0, seed);
+    if (int rc = check_launch("ptar_common_population (draw)")) return rc;
+  }
+  if (!rows || stage == 1) return 0;
+  const int64_t rb = (nreal + ptar::CPOP_RB - 1) / ptar::CPOP_RB;
+  if (rb > 65535) return fail(-3, "ptar_common_population: too many realizations per call%s");
+  const dim3 grid(static_cast<unsigned>((ld + ptar::CPOP_TOAS - 1) / ptar::CPOP_TOAS), static_cast<unsigned>(rb));
+  if (m->K <= 8)
+    ptar::cpop_add_kernel<8><<<grid, ptar::CPOP_TOAS, 0, st>>>(rows, ld, nreal, scratch, m->freqs, m->slot_t, m->slot_psr,
+                                                              m->n_psr, m->K);
+  else if (m->K <= 16)
+    ptar::cpop_add_kernel<16><<<grid, ptar::CPOP_TOAS, 0, st>>>(rows, ld, nreal, scratch, m->freqs, m->slot_t, m->slot_psr,
+                                                               m->n_psr, m->K);
+  else
+    ptar::cpop_add_kernel<32><<<grid, ptar::CPOP_TOAS, 0, st>>>(rows, ld, nreal, scratch, m->freqs, m->slot_t, m->slot_psr,
+                                                               m->n_psr, m->K);
+  return check_launch("ptar_common_population (add)");
+}
+
+int ptar_common_population(double* rows, int64_t ld, int32_t nreal, int64_t real0, uint64_t seed, const ptar_cpop_model* m,
+                           double* scratch, int64_t scratch_len, double* params, void* stream) {
+  return ptar_common_population_stage(rows, ld, nreal, real0, seed, m, scratch, scratch_len, params, 0, stream);
 }
 
 }  // extern "C"

@@ -32,11 +32,6 @@ constexpr int CWP_RB = 16;        // realizations per CTA of the add kernel
 constexpr int CWP_STAGE = 1024;   // doubles of (r, s) records staged in shared memory at once (8 KB)
 constexpr uint32_t K_CWPOP = 7;
 
-// 53-bit uniform in [0, 1) from two Philox words: (a >> 5) 2^26 + (b >> 6), times 2^-53 (exact in fp64).
-__device__ __forceinline__ double uniform53(uint32_t a, uint32_t b) {
-  return static_cast<double>((static_cast<uint64_t>(a >> 5) << 26) | (b >> 6)) * 1.1102230246251565e-16;
-}
-
 // The two uniforms of element `elem` of the population stream for pulsar `psr` (0 except for the pulsar-term phases)
 // and global realization `r`.
 __device__ __forceinline__ void cwpop_uniforms(double u[2], uint32_t elem, uint32_t psr, uint64_t r, const PhiloxKeys& K) {

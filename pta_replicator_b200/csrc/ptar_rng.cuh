@@ -76,13 +76,19 @@ __device__ __forceinline__ void box_muller(uint32_t a, uint32_t b, float& n0, fl
 #endif
 }
 
+// 53-bit uniform in [0, 1) from two Philox words: (a >> 5) 2^26 + (b >> 6), times 2^-53 (exact in fp64).
+__device__ __forceinline__ double uniform53(uint32_t a, uint32_t b) {
+  return static_cast<double>((static_cast<uint64_t>(a >> 5) << 26) | (b >> 6)) * 1.1102230246251565e-16;
+}
+
 // Counter layout: c.x = element index (TOA within the pulsar / ECORR bucket / Fourier column /
 // grid column), c.y = kind | psr << 8, (c.z, c.w) = global realization id >> 2.  The 4 outputs
 // of a counter are the realizations id&~3 .. +3 of that element.
 // The continuous-wave population stream (kind 7, ptar_cwpop.cuh) is keyed per realization instead: c.x = source * 16 +
 // parameter pair (4 = the pulsar-term phase), c.y = 7 | psr << 8 (psr only for that phase), (c.z, c.w) = the full global
 // realization id; its 4 words are two 53-bit uniforms, (w.x >> 5) 2^26 + (w.y >> 6) and (w.z >> 5) 2^26 + (w.w >> 6)
-// times 2^-53.
+// times 2^-53.  The common-process population stream (kind 8, ptar_cpop.cuh) is keyed the same way: c.x = Fourier bin
+// (normals, c.y = 8 | psr << 8) or PTAR_CPOP_HYPER + hyperparameter pair (c.y = 8), (c.z, c.w) = the full realization id.
 __device__ __forceinline__ void normals4(float n[4], uint32_t block, uint32_t kind, uint32_t psr,
                                          uint64_t rfield, const PhiloxKeys& K) {
   const uint4 w = philox4x32_10(make_uint4(block, kind | (psr << 8), static_cast<uint32_t>(rfield),
