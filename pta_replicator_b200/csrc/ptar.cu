@@ -421,6 +421,25 @@ int sky_model_check(const Model* m, bool arrays, const double* sqm, const char* 
   return 0;
 }
 
+// The checks both population entry points share: the call's arguments (-1) and, with rows, the slot table the add stage
+// reads (-2).  Model: ptar_cwpop_model or ptar_cpop_model.
+template <class Model>
+int population_check(const double* rows, int64_t ld, int32_t nreal, int64_t real0, const Model* m, const double* scratch,
+                     int stage, const char* what) {
+  if (!m || !scratch || nreal <= 0 || real0 < 0 || stage < 0 || stage > 2) return fail(-1, "%s: bad argument", what);
+  if (rows && (ld <= 0 || !m->slot_t || !m->slot_psr)) return fail(-2, "%s: rows need ld, slot_t and slot_psr", what);
+  if (!rows && stage == 2) return fail(-2, "%s: the add stage needs rows", what);
+  return 0;
+}
+
+// The grid of a population's add stage: `toas` slots by `rb` realizations per CTA (-3 past 65535 realization blocks).
+int population_add_grid(int64_t ld, int32_t nreal, int toas, int rb, dim3* grid, const char* what) {
+  const int64_t nrb = (int64_t(nreal) + rb - 1) / rb;
+  if (nrb > 65535) return fail(-3, "%s: too many realizations per call", what);
+  *grid = dim3(static_cast<unsigned>((ld + toas - 1) / toas), static_cast<unsigned>(nrb));
+  return 0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1341,7 +1360,7 @@ int ptar_fs_refit(const double* y2, int32_t nreal, const ptar_fs_refit_model* rm
 
 int ptar_cw_population_stage(double* rows, int64_t ld, int32_t nreal, int64_t real0, uint64_t seed, const ptar_cwpop_model* m,
                              double* scratch, int64_t scratch_len, double* params, int stage, void* stream) {
-  if (!m || !scratch || nreal <= 0 || real0 < 0 || stage < 0 || stage > 2) return fail(-1, "ptar_cw_population: bad argument%s");
+  if (int rc = population_check(rows, ld, nreal, real0, m, scratch, stage, "ptar_cw_population")) return rc;
   if (m->n_psr <= 0 || m->n_src < 1 || m->n_src > PTAR_CWPOP_MAX_SRC || m->mode < 0 || m->mode > 2 || !m->phat)
     return fail(-2, "ptar_cw_population: need n_psr >= 1, 1 <= n_src <= 64, mode 0..2 and phat%s");
   if (!m->pphase && !m->pdist) return fail(-2, "ptar_cw_population: pdist missing (no drawn pulsar phase)%s");
@@ -1350,8 +1369,6 @@ int ptar_cw_population_stage(double* rows, int64_t ld, int32_t nreal, int64_t re
   const int64_t pairs = int64_t(nreal) * m->n_src;
   if (scratch_len < pairs * (ptar::CWP_SRC + int64_t(ptar::CWP_PSR) * m->n_psr))
     return fail(-2, "ptar_cw_population: scratch too small (need nreal * n_src * (16 + 8 n_psr) doubles)%s");
-  if (rows && (ld <= 0 || !m->slot_t || !m->slot_psr)) return fail(-2, "ptar_cw_population: rows need ld, slot_t and slot_psr%s");
-  if (!rows && stage == 2) return fail(-2, "ptar_cw_population: the add stage needs rows%s");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   double* src = scratch;
   double* psr = scratch + pairs * ptar::CWP_SRC;
@@ -1362,9 +1379,8 @@ int ptar_cw_population_stage(double* rows, int64_t ld, int32_t nreal, int64_t re
     if (int rc = check_launch("ptar_cw_population (draw)")) return rc;
   }
   if (!rows || stage == 1) return 0;
-  const int64_t rb = (nreal + ptar::CWP_RB - 1) / ptar::CWP_RB;
-  if (rb > 65535) return fail(-3, "ptar_cw_population: too many realizations per call%s");
-  const dim3 grid(static_cast<unsigned>((ld + ptar::CWP_TOAS - 1) / ptar::CWP_TOAS), static_cast<unsigned>(rb));
+  dim3 grid;
+  if (int rc = population_add_grid(ld, nreal, ptar::CWP_TOAS, ptar::CWP_RB, &grid, "ptar_cw_population")) return rc;
   if (m->mode == 0)
     ptar::cwpop_add_kernel<0><<<grid, ptar::CWP_TOAS, 0, st>>>(rows, ld, nreal, src, psr, m->slot_t, m->slot_psr, m->n_psr,
                                                                m->n_src, m->psr_term);
@@ -1385,7 +1401,7 @@ int ptar_cw_population(double* rows, int64_t ld, int32_t nreal, int64_t real0, u
 int ptar_common_population_stage(double* rows, int64_t ld, int32_t nreal, int64_t real0, uint64_t seed,
                                  const ptar_cpop_model* m, double* scratch, int64_t scratch_len, double* params, int stage,
                                  void* stream) {
-  if (!m || !scratch || nreal <= 0 || real0 < 0 || stage < 0 || stage > 2) return fail(-1, "ptar_common_population: bad argument%s");
+  if (int rc = population_check(rows, ld, nreal, real0, m, scratch, stage, "ptar_common_population")) return rc;
   if (m->n_psr < 1 || m->n_psr > PTAR_CPOP_MAX_PSR || m->K < 1 || m->K > PTAR_CPOP_MAX_K || !m->freqs)
     return fail(-2, "ptar_common_population: need 1 <= n_psr <= 2048, 1 <= K <= 32 and freqs%s");
   if (m->spectrum != PTAR_CPOP_POWERLAW && m->spectrum != PTAR_CPOP_FREE) return fail(-2, "ptar_common_population: bad spectrum%s");
@@ -1394,8 +1410,6 @@ int ptar_common_population_stage(double* rows, int64_t ld, int32_t nreal, int64_
     if (m->kind[j] != PTAR_CWPOP_FIXED && m->kind[j] != PTAR_CWPOP_UNIFORM) return fail(-2, "ptar_common_population: bad parameter kind%s");
   const int64_t per_real = int64_t(m->n_psr) * 2 * m->K;
   if (scratch_len < nreal * per_real) return fail(-2, "ptar_common_population: scratch too small (need nreal * n_psr * 2K doubles)%s");
-  if (rows && (ld <= 0 || !m->slot_t || !m->slot_psr)) return fail(-2, "ptar_common_population: rows need ld, slot_t and slot_psr%s");
-  if (!rows && stage == 2) return fail(-2, "ptar_common_population: the add stage needs rows%s");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (stage != 2) {
     const int64_t ctas = int64_t(nreal) * m->K;
@@ -1405,9 +1419,8 @@ int ptar_common_population_stage(double* rows, int64_t ld, int32_t nreal, int64_
     if (int rc = check_launch("ptar_common_population (draw)")) return rc;
   }
   if (!rows || stage == 1) return 0;
-  const int64_t rb = (nreal + ptar::CPOP_RB - 1) / ptar::CPOP_RB;
-  if (rb > 65535) return fail(-3, "ptar_common_population: too many realizations per call%s");
-  const dim3 grid(static_cast<unsigned>((ld + ptar::CPOP_TOAS - 1) / ptar::CPOP_TOAS), static_cast<unsigned>(rb));
+  dim3 grid;
+  if (int rc = population_add_grid(ld, nreal, ptar::CPOP_TOAS, ptar::CPOP_RB, &grid, "ptar_common_population")) return rc;
   if (m->K <= 8)
     ptar::cpop_add_kernel<8><<<grid, ptar::CPOP_TOAS, 0, st>>>(rows, ld, nreal, scratch, m->freqs, m->slot_t, m->slot_psr,
                                                               m->n_psr, m->K);

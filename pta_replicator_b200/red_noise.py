@@ -76,12 +76,16 @@ def add_red_noise(psr: SimulatedPulsar, log10_amplitude: float, spectral_index: 
     batch.set_red(0, log10_amplitude, spectral_index, components=components, modes=modes,
                   libstempo_convention=libstempo_convention)
     J = 2 * len(batch._red["f"][0])
-    z = np.random.randn(J)           # red_noise.py:127
-    torch = batch.torch
-    row = batch.generate(1, inject=dict(zrn=torch.from_numpy(z)[None, None, :]))[0]
+    _add_one(psr, batch, "zrn", np.random.randn(J), "red_noise",   # red_noise.py:127
+             {"amplitude": log10_amplitude, "spectral_index": spectral_index})
+
+
+def _add_one(psr, batch, key, z, suffix, params):
+    """Generate the one-pulsar ``batch`` once with the draws ``z`` injected as ``inject[key]``, add the row to ``psr``'s
+    TOAs and record it as the signal ``<name>_<suffix>`` with ``params``."""
+    row = batch.generate(1, inject={key: batch.torch.from_numpy(z)[None, None, :]})[0]
     dt = TimeArray(batch.unpack(row, 0), "s")
-    psr.update_added_signals("{}_red_noise".format(psr.name),
-                             {"amplitude": log10_amplitude, "spectral_index": spectral_index}, dt)
+    psr.update_added_signals("{}_{}".format(psr.name, suffix), params, dt)
     psr.toas.adjust_TOAs(dt.to("day"))
     psr.update_residuals()
 
@@ -92,14 +96,8 @@ def _add_chromatic(psr, slot, suffix, log10_amplitude, spectral_index, idx, comp
         np.random.seed(seed)
     batch = PulsarBatch([psr], exact_epochs=True)
     batch._set_chrom(slot, 0, log10_amplitude, spectral_index, idx, components, None, fref)
-    z = np.random.randn(2 * components)
-    torch = batch.torch
-    row = batch.generate(1, inject=dict(zchr=torch.from_numpy(z)[None, None, :]))[0]
-    dt = TimeArray(batch.unpack(row, 0), "s")
-    psr.update_added_signals("{}_{}".format(psr.name, suffix),
-                             {"amplitude": log10_amplitude, "spectral_index": spectral_index, "idx": idx, "fref": fref}, dt)
-    psr.toas.adjust_TOAs(dt.to("day"))
-    psr.update_residuals()
+    _add_one(psr, batch, "zchr", np.random.randn(2 * components), suffix,
+             {"amplitude": log10_amplitude, "spectral_index": spectral_index, "idx": idx, "fref": fref})
 
 
 def add_dm_noise(psr: SimulatedPulsar, log10_amplitude: float, spectral_index: float, components: int = 30,
