@@ -67,6 +67,9 @@
  *   ptar_common_population no counterpart (a calibration study draws a common process per realization on the host): a
  *                          power-law or free-spectrum common process, uncorrelated or ORF-correlated, drawn from priors
  *                          on the device in the statistics' Fourier basis and added to every realization
+ *   ptar_transient_        add_gw_memory / add_burst (sine-Gaussian waveforms) per realization with parameters drawn
+ *   population             from priors on the device (a population study calls them once per realization)
+ *                                                                                deterministic.py:718-884
  *   ptar_bwm_sky /         no counterpart (a matched-filter search of add_gw_memory's ramp per realization): the
  *   ptar_bwm_combine       coherent burst-with-memory statistic over epoch x sky and the pulsar-term statistic, reduced
  *                          on the device
@@ -103,7 +106,10 @@ extern "C" {
                              ptar_run_job_to_host_chrom, PTAR_K_CHROM, PTAR_CHROM_SLOTS) and per-realization
                              continuous-wave populations (ptar_cwpop_model, ptar_cw_population[_stage], PTAR_K_CWPOP,
                              PTAR_CWPOP_*) and per-realization common-process populations (ptar_cpop_model,
-                             ptar_common_population[_stage], PTAR_K_CPOP, PTAR_CPOP_*) are new symbols only, so
+                             ptar_common_population[_stage], PTAR_K_CPOP, PTAR_CPOP_*) and per-realization
+                             burst-with-memory and sine-Gaussian burst populations (ptar_tpop_model,
+                             ptar_transient_population[_stage], PTAR_K_BWMPOP, PTAR_K_BURSTPOP, PTAR_TPOP_*)
+                             are new symbols only, so
                              a caller detects them by looking the symbol up.  ptar_os_project accepts nc up to
                              PTAR_RN_MAX_NC since the red-noise likelihood; nothing changes for nc <= PTAR_OS_MAX_NC. */
 
@@ -130,6 +136,8 @@ extern "C" {
 #define PTAR_K_CHROM  6   /* chromatic coefficients: index = (slot << 16) | Fourier column */
 #define PTAR_K_CWPOP  7   /* continuous-wave populations: index = source * 16 + parameter pair, see ptar_cw_population */
 #define PTAR_K_CPOP   8   /* common-process populations: index = bin or PTAR_CPOP_HYPER + pair, see ptar_common_population */
+#define PTAR_K_BWMPOP   9   /* burst-with-memory populations: index = source * 16 + parameter pair, see ptar_transient_population */
+#define PTAR_K_BURSTPOP 10  /* sine-Gaussian burst populations: index = source * 16 + parameter pair, as PTAR_K_BWMPOP */
 
 /* One tile of the packed TOA axis: <=1024 consecutive (time-sorted) TOAs of ONE pulsar
  * touching <=64 kernel-epochs. */
@@ -944,6 +952,69 @@ int ptar_common_population(double* rows, int64_t ld, int32_t nreal, int64_t real
 int ptar_common_population_stage(double* rows, int64_t ld, int32_t nreal, int64_t real0, uint64_t seed,
                                  const ptar_cpop_model* m, double* scratch, int64_t scratch_len, double* params,
                                  int stage, void* stream);
+
+/* Per-realization transient populations (csrc/ptar_tpop.cuh): burst-with-memory (family PTAR_TPOP_BWM) or sine-Gaussian
+ * bursts (PTAR_TPOP_BURST).  Every realization r of [real0, real0 + nreal) gets n_src sources; parameter j is drawn as in
+ * ptar_cw_population (kind PTAR_CWPOP_FIXED: lo, _UNIFORM: lo + width u, _ACOS: acos(lo + width u), each operation of
+ * the affine map rounded once), u the 53-bit uniforms (a >> 5) 2^26 + (b >> 6) times 2^-53 of the Philox4x32-10 words
+ * (a, b) = (w.x, w.y) for even j and (w.z, w.w) for odd j of the counter
+ *   (source * 16 + j / 2, PTAR_K_BWMPOP or PTAR_K_BURSTPOP, r & 0xffffffff, r >> 32).
+ * All PTAR_TPOP_NPAR parameters are drawn whether or not the family uses them; the other streams (kinds 1-8) are
+ * untouched, so every realization's noise and the other populations' draws are what they are without this one, and the
+ * two families never share a uniform.  With t0 = t0_mjd 86400 (rounded once), t = slot_t (MJD 86400), the pattern
+ * (F+, Fx) of add_cgw's formula with 1 + Omega.p = (m.p^2 + n.p^2) / (1 - Omega.p), and (0, 0) where that is below
+ * PTAR_CWPOP_POLE_TOL (or NaN):
+ *   BWM    h = 10^log10_amp, pol = bwm_pol: delay_a(t) = (pol_a h) (t - t0) for t >= t0, else 0, pol_a = cos 2pol F+ +
+ *          sin 2pol Fx (add_gw_memory's Earth-term ramp, deterministic.py:822-884);
+ *   BURST  A = 10^log10_amp, f0 = 10^log10_f0, tau = Q / (2 pi f0), c = cos 2pol, s = sin 2pol (pol = psi):
+ *          delay_a(t) = g (alpha_a cos Phi + beta_a sin Phi), g = exp(-(t - t0)^2 / tau^2), Phi = 2 pi f0 (t - t0) + phase0,
+ *          alpha_a = -A (F+ c + Fx s), beta_a = eps A (F+ s - Fx c): add_burst (deterministic.py:718-793, tref = 0) of
+ *          h+ = A g cos Phi, hx = eps A g sin Phi.  Not truncated: a term is skipped only where g is 0.
+ *   stage 1 (draw)  scratch <- per-(r, s) records [nreal][n_src][4] = {t0 [s], 2 pi f0, 1 / tau, phase0} (BWM: {t0, 0,
+ *                   0, 0}) and per-(r, s, p) coefficients [nreal][n_src][n_psr][2] = {pol_a h, 0} or {alpha_a, beta_a};
+ *                   params (optional) <- [nreal][n_src][PTAR_TPOP_TABLE]:
+ *                     BWM   {t0_mjd, log10_strain, strain, gwtheta, gwphi, bwm_pol, 0 ...}
+ *                     BURST {t0_mjd, log10_amp, amp, log10_f0, f0, Q, tau, gwtheta, gwphi, psi, phase0, eps, a1, a2, a3,
+ *                            a4}, (a1 .. a4) the burst search's amplitudes of this source (its psi = 0, x = 2 pi f0 (t - t0)):
+ *                            a1 = A (c cos phase0 - eps s sin phase0), a2 = A (-c sin phase0 - eps s cos phase0),
+ *                            a3 = A (s cos phase0 + eps c sin phase0), a4 = A (-s sin phase0 + eps c cos phase0).
+ *   stage 2 (add)   rows[r][i] += sum_s delay of source s at slot i for every slot with slot_psr[i] >= 0 whose sum has
+ *                   at least one non-zero term (a slot before every t0 of its realization, or where every g is 0, is
+ *                   not read or written); alignment slots are never touched.
+ * ptar_transient_population runs both (stage 0 of ptar_transient_population_stage); with rows == NULL it only draws.
+ * scratch_len >= nreal * n_src * (4 + 2 n_psr).  Outputs are bit-identical whatever nreal, chunking or real0. */
+#define PTAR_TPOP_BWM      0
+#define PTAR_TPOP_BURST    1
+#define PTAR_TPOP_MAX_SRC  64    /* sources per realization                                               */
+#define PTAR_TPOP_NPAR     10    /* drawn parameters per source (5 counter pairs)                          */
+#define PTAR_TPOP_TABLE    16    /* doubles per (r, s) row of the parameter table                          */
+#define PTAR_TPOP_T0         0   /* parameter indices: the order of the counter's parameter pairs          */
+#define PTAR_TPOP_LOG10_AMP  1   /* log10_strain (BWM) / log10_amp (burst)                                 */
+#define PTAR_TPOP_GWTHETA    2
+#define PTAR_TPOP_GWPHI      3
+#define PTAR_TPOP_POL        4   /* bwm_pol (BWM) / psi (burst)                                            */
+#define PTAR_TPOP_LOG10_F0   5   /* burst only, as are the rest                                            */
+#define PTAR_TPOP_Q          6
+#define PTAR_TPOP_PHASE0     7
+#define PTAR_TPOP_EPS        8   /* index 9: unused                                                        */
+typedef struct {
+  int32_t family;                      /* PTAR_TPOP_BWM / PTAR_TPOP_BURST                                      */
+  int32_t n_psr;                       /* >= 1                                                                 */
+  int32_t n_src;                       /* 1 .. PTAR_TPOP_MAX_SRC                                               */
+  int32_t kind[PTAR_TPOP_NPAR];        /* PTAR_CWPOP_FIXED / _UNIFORM / _ACOS                                  */
+  int32_t reserved;
+  double lo[PTAR_TPOP_NPAR];
+  double width[PTAR_TPOP_NPAR];
+  const double* phat;                  /* [n_psr][3] pulsar unit vectors                                       */
+  const double* slot_t;                /* [ld] TOA (MJD 86400) [s] per slot of the packed axis                 */
+  const int32_t* slot_psr;             /* [ld] pulsar of each slot, -1 for alignment slots (never written)     */
+} ptar_tpop_model;
+
+int ptar_transient_population(double* rows, int64_t ld, int32_t nreal, int64_t real0, uint64_t seed,
+                              const ptar_tpop_model* m, double* scratch, int64_t scratch_len, double* params, void* stream);
+int ptar_transient_population_stage(double* rows, int64_t ld, int32_t nreal, int64_t real0, uint64_t seed,
+                                    const ptar_tpop_model* m, double* scratch, int64_t scratch_len, double* params,
+                                    int stage, void* stream);
 
 /* End-to-end job: GWB mix + synth + generate for realizations [real0, real0+nreal), then
  * (ptar_run_job_to_host) copy the residuals to pinned host memory, chunk by chunk, with the

@@ -54,6 +54,7 @@ def max_red_columns(rc=16, split_epoch=False):
 F_WHITE, F_ECORR, F_RED, F_GWB, F_DET, F_WHITE1 = 1, 2, 4, 8, 16, 32
 TM_KMAX = 32                                       # timing-model columns per pulsar (PTAR_TM_KMAX)
 K_WHITE1, K_WHITE2, K_ECORR, K_RED, K_GWB, K_CHROM, K_CWPOP, K_CPOP = 1, 2, 3, 4, 5, 6, 7, 8
+K_BWMPOP, K_BURSTPOP = 9, 10
 CHROM_SLOTS = 2                                    # chromatic slots of ptar_generate_chrom (PTAR_CHROM_SLOTS)
 
 EXPORTS = ("ptar_version", "ptar_last_error", "ptar_cholesky_lower", "ptar_fourier_basis", "ptar_cgw_delay", "ptar_cw_catalog", "ptar_burst_delay", "ptar_memory_delay",
@@ -65,7 +66,8 @@ EXPORTS = ("ptar_version", "ptar_last_error", "ptar_cholesky_lower", "ptar_fouri
            "ptar_hd_grid", "ptar_rn_grid", "ptar_bwm_sky", "ptar_bwm_combine", "ptar_fs_grid",
            "ptar_burst_ninv", "ptar_burst_project", "ptar_burst_reduce", "ptar_fs_y2", "ptar_fs_refit",
            "ptar_generate_chrom", "ptar_generate_stage_chrom", "ptar_run_job_to_host_chrom",
-           "ptar_cw_population", "ptar_cw_population_stage", "ptar_common_population", "ptar_common_population_stage")
+           "ptar_cw_population", "ptar_cw_population_stage", "ptar_common_population", "ptar_common_population_stage",
+           "ptar_transient_population", "ptar_transient_population_stage")
 OS_MAX_NC, OS_MAX_ORF, OS_MAX_PSR = 32, 4, 256     # optimal statistic: GW-basis columns, templates, pulsars (ptar.h)
 OS_MAX_NULL = 65536                                # null columns of ptar_os_null (PTAR_OS_MAX_NULL)
 OS_NULL_PHASE_SHIFT, OS_NULL_SKY_SCRAMBLE = 1, 2
@@ -86,6 +88,9 @@ CWPOP_SRC, CWPOP_PSR = 16, 8                       # doubles per (r, s) and per 
 CWPOP_FIXED, CWPOP_UNIFORM, CWPOP_ACOS = 0, 1, 2   # parameter kinds of ptar_cwpop_model
 CPOP_MAX_K, CPOP_MAX_PSR, CPOP_HYPER = 32, 2048, 0x10000   # common-process populations: bins, pulsars, hyper counters
 CPOP_POWERLAW, CPOP_FREE = 0, 1                    # spectra of ptar_cpop_model
+TPOP_BWM, TPOP_BURST = 0, 1                        # families of ptar_tpop_model
+TPOP_MAX_SRC, TPOP_NPAR, TPOP_TABLE = 64, 10, 16   # transient populations: sources per realization, parameters, table row
+TPOP_REC, TPOP_COEF = 4, 2                         # doubles per (r, s) and per (r, s, p) record of the scratch (ptar_tpop.cuh)
 BWM_LINV = 6                                       # packed L2^-1 doubles per (epoch pair, sky point) (csrc/ptar_bwm.cuh)
 
 
@@ -223,6 +228,12 @@ class CpopModel(C.Structure):
                 ("slot_t", C.c_void_p), ("slot_psr", C.c_void_p)]
 
 
+class TpopModel(C.Structure):
+    _fields_ = [("family", C.c_int32), ("n_psr", C.c_int32), ("n_src", C.c_int32), ("kind", C.c_int32 * TPOP_NPAR),
+                ("reserved", C.c_int32), ("lo", C.c_double * TPOP_NPAR), ("width", C.c_double * TPOP_NPAR),
+                ("phat", C.c_void_p), ("slot_t", C.c_void_p), ("slot_psr", C.c_void_p)]
+
+
 _lib = None
 
 
@@ -300,6 +311,8 @@ def lib():
     L.ptar_cw_population_stage.argtypes = [vp, i64, C.c_int32, i64, u64, vp, vp, i64, vp, i32, vp]
     L.ptar_common_population.argtypes = [vp, i64, C.c_int32, i64, u64, vp, vp, i64, vp, vp]   # m: address of a CpopModel
     L.ptar_common_population_stage.argtypes = [vp, i64, C.c_int32, i64, u64, vp, vp, i64, vp, i32, vp]
+    L.ptar_transient_population.argtypes = [vp, i64, C.c_int32, i64, u64, vp, vp, i64, vp, vp]   # m: address of a TpopModel
+    L.ptar_transient_population_stage.argtypes = [vp, i64, C.c_int32, i64, u64, vp, vp, i64, vp, i32, vp]
     for name in EXPORTS:
         if name not in ("ptar_version", "ptar_last_error"):
             getattr(L, name).restype = C.c_int

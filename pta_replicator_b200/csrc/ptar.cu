@@ -29,6 +29,7 @@
 #include "ptar_rn.cuh"
 #include "ptar_rng.cuh"
 #include "ptar_timing.cuh"
+#include "ptar_tpop.cuh"
 
 namespace {
 
@@ -421,8 +422,8 @@ int sky_model_check(const Model* m, bool arrays, const double* sqm, const char* 
   return 0;
 }
 
-// The checks both population entry points share: the call's arguments (-1) and, with rows, the slot table the add stage
-// reads (-2).  Model: ptar_cwpop_model or ptar_cpop_model.
+// The checks every population entry point shares: the call's arguments (-1) and, with rows, the slot table the add stage
+// reads (-2).  Model: ptar_cwpop_model, ptar_cpop_model or ptar_tpop_model.
 template <class Model>
 int population_check(const double* rows, int64_t ld, int32_t nreal, int64_t real0, const Model* m, const double* scratch,
                      int stage, const char* what) {
@@ -1436,6 +1437,44 @@ int ptar_common_population_stage(double* rows, int64_t ld, int32_t nreal, int64_
 int ptar_common_population(double* rows, int64_t ld, int32_t nreal, int64_t real0, uint64_t seed, const ptar_cpop_model* m,
                            double* scratch, int64_t scratch_len, double* params, void* stream) {
   return ptar_common_population_stage(rows, ld, nreal, real0, seed, m, scratch, scratch_len, params, 0, stream);
+}
+
+int ptar_transient_population_stage(double* rows, int64_t ld, int32_t nreal, int64_t real0, uint64_t seed,
+                                    const ptar_tpop_model* m, double* scratch, int64_t scratch_len, double* params, int stage,
+                                    void* stream) {
+  if (int rc = population_check(rows, ld, nreal, real0, m, scratch, stage, "ptar_transient_population")) return rc;
+  if (m->family != PTAR_TPOP_BWM && m->family != PTAR_TPOP_BURST) return fail(-2, "ptar_transient_population: bad family%s");
+  if (m->n_psr <= 0 || m->n_src < 1 || m->n_src > PTAR_TPOP_MAX_SRC || !m->phat)
+    return fail(-2, "ptar_transient_population: need n_psr >= 1, 1 <= n_src <= 64 and phat%s");
+  for (int j = 0; j < PTAR_TPOP_NPAR; ++j)
+    if (m->kind[j] < PTAR_CWPOP_FIXED || m->kind[j] > PTAR_CWPOP_ACOS)
+      return fail(-2, "ptar_transient_population: bad parameter kind%s");
+  const int64_t pairs = int64_t(nreal) * m->n_src;
+  if (scratch_len < pairs * (ptar::TP_REC + int64_t(ptar::TP_COEF) * m->n_psr))
+    return fail(-2, "ptar_transient_population: scratch too small (need nreal * n_src * (4 + 2 n_psr) doubles)%s");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  double* rec = scratch;
+  double* coef = scratch + pairs * ptar::TP_REC;
+  if (stage != 2) {
+    ptar::tpop_draw_kernel<<<static_cast<unsigned>((pairs + 127) / 128), 128, 0, st>>>(rec, coef, params, *m, nreal, real0,
+                                                                                       seed);
+    if (int rc = check_launch("ptar_transient_population (draw)")) return rc;
+  }
+  if (!rows || stage == 1) return 0;
+  dim3 grid;
+  if (int rc = population_add_grid(ld, nreal, ptar::TP_TOAS, ptar::TP_RB, &grid, "ptar_transient_population")) return rc;
+  if (m->family == PTAR_TPOP_BWM)
+    ptar::tpop_add_kernel<PTAR_TPOP_BWM><<<grid, ptar::TP_TOAS, 0, st>>>(rows, ld, nreal, rec, coef, m->slot_t, m->slot_psr,
+                                                                         m->n_psr, m->n_src);
+  else
+    ptar::tpop_add_kernel<PTAR_TPOP_BURST><<<grid, ptar::TP_TOAS, 0, st>>>(rows, ld, nreal, rec, coef, m->slot_t,
+                                                                           m->slot_psr, m->n_psr, m->n_src);
+  return check_launch("ptar_transient_population (add)");
+}
+
+int ptar_transient_population(double* rows, int64_t ld, int32_t nreal, int64_t real0, uint64_t seed, const ptar_tpop_model* m,
+                              double* scratch, int64_t scratch_len, double* params, void* stream) {
+  return ptar_transient_population_stage(rows, ld, nreal, real0, seed, m, scratch, scratch_len, params, 0, stream);
 }
 
 }  // extern "C"

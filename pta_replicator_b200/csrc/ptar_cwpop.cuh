@@ -32,10 +32,11 @@ constexpr int CWP_RB = 16;        // realizations per CTA of the add kernel
 constexpr int CWP_STAGE = 1024;   // doubles of (r, s) records staged in shared memory at once (8 KB)
 constexpr uint32_t K_CWPOP = 7;
 
-// The two uniforms of element `elem` of the population stream for pulsar `psr` (0 except for the pulsar-term phases)
-// and global realization `r`.
-__device__ __forceinline__ void cwpop_uniforms(double u[2], uint32_t elem, uint32_t psr, uint64_t r, const PhiloxKeys& K) {
-  const uint4 w = philox4x32_10(make_uint4(elem, K_CWPOP | (psr << 8), static_cast<uint32_t>(r), static_cast<uint32_t>(r >> 32)), K);
+// The two uniforms of element `elem` of the population stream `kind` (PTAR_K_CWPOP, or a transient population's) for
+// pulsar `psr` (0 except for the pulsar-term phases) and global realization `r`.
+__device__ __forceinline__ void cwpop_uniforms(double u[2], uint32_t elem, uint32_t psr, uint64_t r, const PhiloxKeys& K,
+                                               uint32_t kind = K_CWPOP) {
+  const uint4 w = philox4x32_10(make_uint4(elem, kind | (psr << 8), static_cast<uint32_t>(r), static_cast<uint32_t>(r >> 32)), K);
   u[0] = uniform53(w.x, w.y);
   u[1] = uniform53(w.z, w.w);
 }

@@ -89,6 +89,8 @@ __device__ __forceinline__ double uniform53(uint32_t a, uint32_t b) {
 // realization id; its 4 words are two 53-bit uniforms, (w.x >> 5) 2^26 + (w.y >> 6) and (w.z >> 5) 2^26 + (w.w >> 6)
 // times 2^-53.  The common-process population stream (kind 8, ptar_cpop.cuh) is keyed the same way: c.x = Fourier bin
 // (normals, c.y = 8 | psr << 8) or PTAR_CPOP_HYPER + hyperparameter pair (c.y = 8), (c.z, c.w) = the full realization id.
+// The transient population streams (kinds 9 and 10, ptar_tpop.cuh) are keyed as kind 7: c.x = source * 16 + parameter
+// pair, c.y = 9 (burst with memory) or 10 (sine-Gaussian burst), (c.z, c.w) = the full realization id.
 __device__ __forceinline__ void normals4(float n[4], uint32_t block, uint32_t kind, uint32_t psr,
                                          uint64_t rfield, const PhiloxKeys& K) {
   const uint4 w = philox4x32_10(make_uint4(block, kind | (psr << 8), static_cast<uint32_t>(rfield),
