@@ -64,21 +64,51 @@ def ld_phi(freqs, gamma, Tspan, log10_A=None):
     return p if log10_A is None else p * LD(10) ** (2 * LD(log10_A))
 
 
-def covariance(b, i, common=None):
-    """P_a [n, n] (long double): white + ECORR + red noise (+ common: (basis [n, m] fp64, prior [m] long double))."""
+def covariance(b, i, common=None, own_red=True):
+    """P_a [n, n] (long double): white + ECORR + red noise (left out with ``own_red`` False) + every chromatic process
+    (w w^T) ⊙ (F_s phi_s F_s^T) (+ common: (basis [n, m] fp64, prior [m] long double))."""
     w1, w2 = (np.asarray(v, dtype=float).astype(LD) for v in b._white[i])
     P = np.diag(w1 * w1 + w2 * w2)
     if b._ecorr is not None and b._ecorr[i] is not None:
         bucket, e = b._ecorr[i]
         e2 = np.asarray(e, dtype=float).astype(LD)[bucket] ** 2
         P = P + np.where(bucket[:, None] == bucket[None, :], e2[:, None], LD(0))
-    if b._red is not None and b._red["f"][i] is not None:
+    if own_red and b._red is not None and b._red["f"][i] is not None:
         Fr = basis(b.t_tdb[i], b._red["f"][i]).astype(LD)
         P = P + (Fr * np.asarray(b._red["scale"][i], dtype=float).astype(LD) ** 2) @ Fr.T
+    for Fw, phi in chrom_blocks(b, i):
+        P = P + (Fw * phi) @ Fw.T
     if common is not None:
         Fc = common[0].astype(LD)
         P = P + (Fc * common[1]) @ Fc.T
     return P
+
+
+def radio_freq(b, i):
+    """The TOAs' radio frequencies [MHz] of pulsar ``i`` in engine order, read from its TOA table."""
+    col = b.psrs[i].toas.table["freq"]
+    return np.asarray(getattr(col, "value", col), dtype=float)[b.order[i]]
+
+
+def chrom_blocks(b, i):
+    """Per chromatic process of pulsar ``i``: (w ⊙ F_s [n, J] long double, phi_s [J] long double) with the weight
+    restated from its definition, w = (fref / nu)^idx on the table's radio frequencies, (idx, fref) as recorded by
+    ``Edge.dm`` / ``Edge.chrom`` (or set in ``b._ref_chrom[(slot, i)]`` by the caller: a process without a record is an
+    error, not an assumed default); the frequencies and sqrt-priors are the recipe's fp64 parameters, as for the red
+    noise."""
+    out = []
+    rec = getattr(b, "_ref_chrom", {})
+    for slot, c in enumerate(getattr(b, "_chrom", ())):
+        if c is None or c["f"][i] is None:
+            continue
+        if (slot, i) not in rec:
+            raise ValueError(f"chromatic slot {slot} of pulsar {i} has no recorded (idx, fref): register it through "
+                             "Edge.dm / Edge.chrom or record it in b._ref_chrom")
+        idx, fref = rec[(slot, i)]
+        w = (LD(fref) / radio_freq(b, i).astype(LD)) ** LD(idx)
+        out.append((w[:, None] * basis(b.t_tdb[i], c["f"][i]).astype(LD),
+                    np.asarray(c["scale"][i], dtype=float).astype(LD) ** 2))
+    return out
 
 
 def ld_cholesky(A):
@@ -116,16 +146,16 @@ def spd_solve(A, B, L=None, steps=2):
 
 
 def design(b, i, tm):
-    """The timing design matrix [n, k] (engine order, fp64) of ``tm`` = dict(poly, jumps, extra), or None: the columns
-    ``set_timing_model`` documents (1, x, .., x^poly in x = (t - t_mid) / (t_span / 2); one indicator per flag value,
-    the earliest group dropped with a polynomial; ``extra`` in table order)."""
+    """The timing design matrix [n, k] (engine order, fp64) of ``tm`` = dict(poly, jumps, extra, dm), or None: the
+    columns ``set_timing_model`` documents (1, x, .., x^poly in x = (t - t_mid) / (t_span / 2); one indicator per flag
+    value, the earliest group dropped with a polynomial; ``extra`` in table order; (1400 / nu)^2 x^d, d = 0..dm)."""
     if tm is None:
         return None
     t, n = b.t_tdb[i], b.ntoa[i]
     cols = []
+    half = 0.5 * (t.max() - t.min())
+    x = (t - 0.5 * (t.max() + t.min())) / half
     if tm.get("poly") is not None:
-        half = 0.5 * (t.max() - t.min())
-        x = (t - 0.5 * (t.max() + t.min())) / half
         cols += [x ** d for d in range(int(tm["poly"]) + 1)]
     if tm.get("jumps") is not None:
         fl = b.psrs[i].toas.table["flags"]
@@ -136,16 +166,25 @@ def design(b, i, tm):
     if tm.get("extra") is not None:
         ex = np.asarray(tm["extra"], dtype=float).reshape(n, -1)
         cols += list(ex[b.order[i]].T)
+    if tm.get("dm") is not None:
+        w = (1400.0 / radio_freq(b, i)) ** 2
+        cols += [w * x ** d for d in range(int(tm["dm"]) + 1)]
     return np.stack(cols, axis=1) if cols else None
 
 
-def tier1(b, i, F, common=None, tm=None):
+def tier1(b, i, F, common=None, tm=None, own_red=True):
     """C_a [n, m] = P_a^-1 F with the timing model ``tm`` marginalised (constrained form), long double; in mpmath for
     pulsars of at most MP_TOAS TOAs, where a timing model that takes all but a few TOAs makes C_a a difference of
-    terms up to 1e17 times larger."""
+    terms up to 1e17 times larger.  ``own_red`` as for ``covariance``."""
     if b.ntoa[i] <= MP_TOAS:
-        return _tier1_mp(b, i, F, common, tm)
-    A = covariance(b, i, common)
+        return _tier1_mp(b, i, F, common, tm, own_red)
+    return dense_pinv(b, i, F, common, tm, own_red)
+
+
+def dense_pinv(b, i, F, common=None, tm=None, own_red=True):
+    """P_a^-1 F in long double (Cholesky of the dense ``covariance``, two steps of refinement per solve) with the timing
+    model ``tm`` marginalised in the constrained form."""
+    A = covariance(b, i, common, own_red)
     L = ld_cholesky(A)
     M = design(b, i, tm)
     if M is None:
@@ -161,9 +200,9 @@ def tier1(b, i, F, common=None, tm=None):
 MP_TOAS = 16
 
 
-def _tier1_mp(b, i, F, common, tm):
+def _tier1_mp(b, i, F, common, tm, own_red=True):
     with mp.workdps(DPS):
-        A = mp.matrix(mpmat(covariance(b, i, common)))
+        A = mp.matrix(mpmat(covariance(b, i, common, own_red)))
         Fm = mp.matrix(mpmat(F))
         M = design(b, i, tm)
         PF = _m_lu(A, Fm)
@@ -179,17 +218,21 @@ def _tier1_mp(b, i, F, common, tm):
     return out
 
 
-def woodbury_cond(b, i, common=None, tm=None):
-    """kappa_2 of the unit-diagonal S = Phi^-1 + T^T N^-1 T, T = [M, F_red, F_common], Phi^-1 = [0, 1/phi_red,
-    1/phi_common] (1 without any block): the conditioning of the system the product's Woodbury form solves."""
+def woodbury_cond(b, i, common=None, tm=None, own_red=True):
+    """kappa_2 of the unit-diagonal S = Phi^-1 + T^T N^-1 T, T = [M, F_red, w ⊙ F_chromatic.., F_common], Phi^-1 =
+    [0, 1/phi_red, 1/phi_chromatic.., 1/phi_common] (1 without any block): the conditioning of the system the
+    product's Woodbury form solves.  ``own_red`` as for ``covariance``."""
     blocks, ip = [], []
     M = design(b, i, tm)
     if M is not None:
         blocks.append(M)
         ip.append(np.zeros(M.shape[1], dtype=LD))
-    if b._red is not None and b._red["f"][i] is not None:
+    if own_red and b._red is not None and b._red["f"][i] is not None:
         blocks.append(basis(b.t_tdb[i], b._red["f"][i]))
         ip.append(1 / np.asarray(b._red["scale"][i], dtype=float).astype(LD) ** 2)
+    for Fw, phi in chrom_blocks(b, i):
+        blocks.append(Fw)
+        ip.append(1 / phi)
     if common is not None:
         blocks.append(common[0])
         ip.append(1 / common[1])
@@ -202,27 +245,28 @@ def woodbury_cond(b, i, common=None, tm=None):
     return float(np.linalg.cond((S * sc[:, None] * sc[None, :]).astype(np.float64)))
 
 
-def cancellation_cond(e, K, Tspan):
-    """max over pulsars of max|F^T N^-1 F| / min_j Z_a,jj (long double; GW basis k / Tspan, k = 1..K): how far the
-    red-noise and timing-model terms the product subtracts from N^-1 F (Woodbury, then the projection) cancel it."""
+def cancellation_cond(e, K, Tspan, own_red=True):
+    """max over pulsars of max|F^T N^-1 F| / min_j Z_a,jj (long double; GW basis k / Tspan, k = 1..K, ``Tspan`` one
+    value or one per pulsar): how far the red-noise, chromatic and timing-model terms the product subtracts from
+    N^-1 F (Woodbury, then the projection) cancel it.  ``own_red`` as for ``covariance``."""
     b = e.b
-    f = np.arange(1, K + 1) / Tspan
     out = 0.0
     for i in range(b.n_psr):
-        F = basis(b.t_tdb[i], f)
+        F = basis(b.t_tdb[i], np.arange(1, K + 1) / (Tspan[i] if np.ndim(Tspan) else Tspan))
         Zn = F.astype(LD).T @ spd_solve(noise_cov(b, i), F.astype(LD), steps=0)
-        Z = F.astype(LD).T @ tier1(b, i, F, None, e.tm[i])
+        Z = F.astype(LD).T @ tier1(b, i, F, None, e.tm[i], own_red)
         out = max(out, float(np.max(np.abs(Zn)) / np.min(np.abs(np.diag(Z)))))
     return out
 
 
 def noise_cov(b, i):
     """N_a: white + ECORR only (long double)."""
-    red, b._red = b._red, None
+    red, chrom = b._red, b._chrom
+    b._red, b._chrom = None, ()
     try:
         return covariance(b, i)
     finally:
-        b._red = red
+        b._red, b._chrom = red, chrom
 
 
 # ------------------------------------------------------------------ tier 2: mpmath
@@ -463,6 +507,97 @@ def optimal_statistic(e, rows):
     return out
 
 
+def pfos(e, rows):
+    """dict(rho [R, K, n_pairs], phi, snr, phi_mc [R, n_orf, K], their scales, t [K, n_pairs], D [n_orf, K]) of the
+    per-frequency optimal statistic on ``e.stats["os"]``, in the units of the unscaled projection: Z_a[k] the 2 x 2
+    diagonal block of Z_a at f_k, X_a,k the projection pair, t_qk = tr(Z_a[k] Z_b[k]), d_qk = X_a,k . X_b,k,
+    D_ok = sum_q (Gamma^o_q)^2 t_qk, (F_k)_oo' = sum_q Gamma^o_q Gamma^o'_q t_qk; scales |X_a,k||X_b,k| and their
+    template sums, as ``optimal_statistic``."""
+    o, b = e.stats["os"], e.b
+    Tspan = array_tspan(b, o["Tspan"])
+    _, t1 = _gw_tier1(e, rows, o["K"], Tspan, o["log10_A_common"], o["gamma"])
+    K, P, R = o["K"], b.n_psr, rows.shape[0]
+    pa, pb = np.triu_indices(P, 1)
+    nq, no = len(pa), len(o["orfs"])
+    out = {k: np.zeros((R, K, nq)) for k in ("rho", "rho_s")}
+    out.update({k: np.zeros((R, no, K)) for k in ("phi", "phi_s", "snr", "snr_s", "phi_mc", "phi_mc_s")})
+    tt, DD = np.zeros((K, nq)), np.zeros((no, K))
+    with mp.workdps(DPS):
+        W = [[Gm[a][c] for a, c in zip(pa, pb)] for Gm in (m_orf(b, g) for g in o["orfs"])]
+        Zm = [mpmat(z) for _, z, _ in t1]
+        Xm = [[mpvec(r) for r in X] for _, _, X in t1]
+        for k in range(K):
+            c2 = (2 * k, 2 * k + 1)
+            t = [mp.fsum(Zm[a][u][v] * Zm[c][v][u] for u in c2 for v in c2) for a, c in zip(pa, pb)]
+            D = [mp.fsum(w[q] ** 2 * t[q] for q in range(nq)) for w in W]
+            Fi = mp.matrix([[mp.fsum(W[i][q] * W[j][q] * t[q] for q in range(nq)) for j in range(no)]
+                            for i in range(no)]) ** -1
+            tt[k], DD[:, k] = [float(v) for v in t], [float(v) for v in D]
+            for r in range(R):
+                d = [mp.fsum(Xm[a][r][u] * Xm[c][r][u] for u in c2) for a, c in zip(pa, pb)]
+                nx = [mp.sqrt(mp.fsum(Xm[a][r][u] ** 2 for u in c2)) for a in range(P)]
+                dn = [nx[a] * nx[c] for a, c in zip(pa, pb)]
+                bo = [mp.fsum(W[i][q] * d[q] for q in range(nq)) for i in range(no)]
+                bs = [mp.fsum(abs(W[i][q]) * dn[q] for q in range(nq)) for i in range(no)]
+                out["rho"][r, k] = [float(d[q] / t[q]) for q in range(nq)]
+                out["rho_s"][r, k] = [float(dn[q] / t[q]) for q in range(nq)]
+                for i in range(no):
+                    out["phi"][r, i, k], out["phi_s"][r, i, k] = float(bo[i] / D[i]), float(bs[i] / D[i])
+                    out["snr"][r, i, k], out["snr_s"][r, i, k] = float(bo[i] / mp.sqrt(D[i])), float(bs[i] / mp.sqrt(D[i]))
+                    out["phi_mc"][r, i, k] = float(mp.fsum(Fi[i, j] * bo[j] for j in range(no)))
+                    out["phi_mc_s"][r, i, k] = float(mp.fsum(abs(Fi[i, j]) * bs[j] for j in range(no)))
+    out.update(t=tt, D=DD)
+    return out
+
+
+def rn_spans(e):
+    """T_a per pulsar of ``e.stats["rn"]``: its Tspan, else the pulsar's own span."""
+    o, b = e.stats["rn"], e.b
+    return [float(o["Tspan"]) if o["Tspan"] is not None else float(t.max() - t.min()) for t in b.t_tdb]
+
+
+def rn(e, rows, given=None):
+    """dict(lnl [R, P, Ng, NA], ldet [P, Ng, NA], scale = 1 + Q/2 + ldet/2, C, Z [P, 2K, 2K]) of the red-noise
+    likelihood ``e.stats["rn"]``: per pulsar the basis F_a at k / T_a, C_a = P_a^-1 F_a with the pulsar's own red noise
+    out of P_a (its chromatic processes and the optional common power law at k / Tspan of the array in it), Z_a =
+    F_a^T C_a, X_a = C_a^T r, and per grid point ln L_a = 1/2 y^T (I + M)^-1 y - 1/2 ln det(I + M), M = A^2 phi~^1/2
+    Z_a phi~^1/2, y = A phi~^1/2 X_a (phi~ the set_red power law at T_a); ``given`` as for ``curn``."""
+    o, b = e.stats["rn"], e.b
+    x, gam = o["log10_A"], o["gamma"]
+    P, R, nc = b.n_psr, rows.shape[0], 2 * o["K"]
+    TA = array_tspan(b)
+    fc = np.arange(1, o["components_common"] + 1) / TA
+    lnl, Q = np.zeros((R, P, len(gam), len(x))), np.zeros((R, P, len(gam), len(x)))
+    ldet = np.zeros((P, len(gam), len(x)))
+    Cs, Zs = [], []
+    with mp.workdps(DPS):
+        for i, Ta in enumerate(rn_spans(e)):
+            f = np.arange(1, o["K"] + 1) / Ta
+            F = basis(b.t_tdb[i], f)
+            common = None if o["log10_A_common"] is None else \
+                (basis(b.t_tdb[i], fc), ld_phi(fc, o["gamma_common"], TA, o["log10_A_common"]))
+            C = tier1(b, i, F, common, e.tm[i], own_red=False) if given is None else \
+                np.asarray(given[i], dtype=np.float64).astype(LD)
+            Z, X = F.astype(LD).T @ C, _rows_of(b, rows, i) @ C
+            Cs.append(C)
+            Zs.append(Z)
+            Zm, Xm = mpmat(Z), [mpvec(r) for r in X]
+            for g, gm in enumerate(gam):
+                sp = [mp.sqrt(v) for v in m_phi(f, gm, Ta)]
+                Zh = [[sp[j] * Zm[j][k] * sp[k] for k in range(nc)] for j in range(nc)]
+                Xh = [[sp[j] * r[j] for j in range(nc)] for r in Xm]
+                for k, xa in enumerate(x):
+                    a2 = mp.mpf(10) ** (2 * mpf(xa))
+                    L = m_chol([[(1 if j == c else 0) + a2 * Zh[j][c] for c in range(nc)] for j in range(nc)])
+                    ld = m_logdet(L)
+                    ldet[i, g, k] = float(ld)
+                    for r in range(R):
+                        q = a2 * mp.fsum(u * v for u, v in zip(Xh[r], m_solve(L, Xh[r])))
+                        lnl[r, i, g, k] = float(q / 2 - ld / 2)
+                        Q[r, i, g, k] = float(q)
+    return dict(lnl=lnl, ldet=ldet, scale=1 + 0.5 * Q + 0.5 * ldet[None], C=Cs, Z=np.stack(Zs).astype(np.float64))
+
+
 def anisotropy(e, rows, templates_sph=None):
     """dict(clm [R, n_lm], chi2 [R], radio [R, S] and their scales) of ``e.stats["aniso"]`` (lmax, sky) on the optimal
     statistic: F = T diag(t) T^T, c = F^-1 T d, chi2 = y^T F^-1 y - y_0^2 / F_00 (y = T d), S/N_k = y_k / sqrt(F_kk).
@@ -617,12 +752,41 @@ class Edge:
         from pta_replicator_b200.engine import PulsarBatch
         self.name = name
         self.b = PulsarBatch(psrs, plan_only=PLAN_ONLY)
+        self.b._ref_chrom = {}
         self.tm = [None] * self.b.n_psr
         self.stats = {}
 
-    def timing_model(self, i, poly=2, jumps=None, extra=None):
-        self.b.set_timing_model(i, poly=poly, jumps=jumps, extra=extra)
-        self.tm[i] = dict(poly=poly, jumps=jumps, extra=extra)
+    def timing_model(self, i, poly=2, jumps=None, extra=None, dm=None):
+        self.b.set_timing_model(i, poly=poly, jumps=jumps, extra=extra, dm=dm)
+        self.tm[i] = dict(poly=poly, jumps=jumps, extra=extra, dm=dm)
+
+    def dm(self, i, log10_A, gamma, components, modes=None, fref=1400.0):
+        """DM noise on pulsar ``i``; the reference restates its weight from (idx = 2, ``fref``)."""
+        self.b.set_dm_noise(i, log10_A, gamma, components=components, modes=modes, fref=fref)
+        self.b._ref_chrom[(0, i)] = (2.0, fref)
+        return self
+
+    def chrom(self, i, log10_A, gamma, components, idx=4.0, modes=None, fref=1400.0):
+        """A chromatic (scattering, idx 4) process on pulsar ``i``; the reference restates its weight from (idx, fref)."""
+        self.b.set_chromatic_noise(i, log10_A, gamma, idx=idx, components=components, modes=modes, fref=fref)
+        self.b._ref_chrom[(1, i)] = (float(idx), fref)
+        return self
+
+    def rn(self, K, log10_A=(-15.0, -12.5, -11.0), gamma=(1.0, 4.0, 6.5), Tspan=None, log10_A_common=None,
+           gamma_common=13 / 3, components_common=14):
+        """The red-noise likelihood on a 3 x 3 grid, optionally with a common power law in P_a."""
+        x, g = np.array(log10_A, dtype=float), np.array(gamma, dtype=float)
+        self.b.set_red_noise_likelihood(log10_A=x, gamma=g, components=K, Tspan=Tspan, log10_A_common=log10_A_common,
+                                        gamma_common=gamma_common, components_common=components_common)
+        self.stats["rn"] = dict(K=K, log10_A=x, gamma=g, Tspan=Tspan, log10_A_common=log10_A_common,
+                                gamma_common=gamma_common, components_common=components_common)
+        return self
+
+    def pfos(self):
+        """The per-frequency optimal statistic on the ``os`` registration."""
+        self.b.set_os_per_frequency()
+        self.stats["os"]["pf"] = True
+        return self
 
     def curn(self, K, log10_A=(-18.0, -12.0, -11.0), gamma=(0.0, 7.0), Tspan=None, hd=None):
         x, g = np.array(log10_A, dtype=float), np.array(gamma, dtype=float)
@@ -655,10 +819,13 @@ class Edge:
         return self
 
 
-def pulsars(ntoas, seed=0, err_us=None, pos=None, jump_single=False, name="T"):
+def pulsars(ntoas, seed=0, err_us=None, pos=None, jump_single=False, name="T", radio=False, single=(), spans={}):
     """Synthetic pulsars with the given TOA counts: epochs of 1-4 TOAs within 1 s over MJD 53000-58800, backends A/B/C
     cycling per epoch (flag f), uncertainties 0.3-3 us (or ``err_us(rng, n)``), isotropic positions (or ``pos``:
-    (RAJ [h], DECJ [deg]) per pulsar).  ``jump_single``: flag j = "x" on every TOA but one (index n // 2, "y")."""
+    (RAJ [h], DECJ [deg]) per pulsar).  ``jump_single``: flag j = "x" on every TOA but one (index n // 2, "y").
+    ``radio``: sub-band radio frequencies, each epoch's TOAs spread evenly over 700-1900 MHz (1400 MHz alone), the
+    pulsars in ``single`` at 820 MHz only; they draw nothing, so the TOAs are those of ``radio`` False.  ``spans``:
+    pulsar -> (first, last) MJD range of its epochs instead of 53000-58800."""
     from pta_replicator_b200.simulate import make_ideal, pulsar_from_arrays
     rng = np.random.default_rng(seed)
     out = []
@@ -666,14 +833,18 @@ def pulsars(ntoas, seed=0, err_us=None, pos=None, jump_single=False, name="T"):
         sub = []
         while sum(sub) < n:
             sub.append(int(min(rng.integers(1, 5), n - sum(sub))))
-        ep = np.sort(rng.uniform(53000.0, 58800.0, len(sub)))
+        ep = np.sort(rng.uniform(*spans.get(j, (53000.0, 58800.0)), len(sub)))
         mjd = np.concatenate([e + np.sort(rng.uniform(0, 0.9, k)) / 86400.0 for e, k in zip(ep, sub)])
         be = np.concatenate([[("A", "B", "C")[q % 3]] * k for q, k in enumerate(sub)])
         ra, dec = (rng.uniform(0, 24), math.degrees(math.asin(rng.uniform(-1, 1)))) if pos is None else pos[j]
         err = rng.uniform(0.3, 3.0, n) if err_us is None else err_us(rng, n)
         fl = [{"f": f, "j": "y" if (jump_single and q == n // 2) else "x"} for q, f in enumerate(be)]
+        kw = {}
+        if radio:
+            nu = np.concatenate([np.linspace(700.0, 1900.0, k) if k > 1 else [1400.0] for k in sub])
+            kw["freq"] = np.full(n, 820.0) if j in single else nu
         p = pulsar_from_arrays(f"{name}{j:03d}", {"RAJ": float(ra), "DECJ": float(dec)}, mjd.astype(np.longdouble), err,
-                               flags=fl)
+                               flags=fl, **kw)
         make_ideal(p)
         out.append(p)
     return out
@@ -846,6 +1017,54 @@ def recipes():
         e = _noise(Edge("aniso_lmax1", pulsars((5, 7, 65, 193, 30, 40), 95)), tm=True)
         return e.os(4, orfs=("hd",), lmax=1, sky=[[0.4, 0.2], [2.0, 3.0]])
     R["aniso_lmax1"] = aniso
+
+    # 10. chromatic noise: DM (idx 2) and scattering (idx 4) processes in every statistic's P_a
+    def chrom_all():
+        e = _noise(Edge("chrom_all", pulsars(EDGE4, 101, radio=True)), red=(-14.0, 4.0, 8))
+        for i in range(e.b.n_psr):
+            e.dm(i, -13.3, 2.5, 8)
+            if e.b.ntoa[i] >= 20:
+                e.chrom(i, -13.8, 3.0, 5)
+                e.timing_model(i, poly=2, jumps="f", dm=1)
+        return e.curn(4, hd="hd").os(4, orfs=("hd", "monopole")).pfos().fp(n_freqs=3, sky=[[0.4, 1.2], [2.2, 4.4]]).rn(4)
+    R["chrom_all"] = chrom_all
+
+    def chrom_single_freq():
+        # pulsar 2 observes at 820 MHz only, with loud red and DM noise on the same frequencies: its two T blocks are
+        # scaled copies and S is regularised only by Phi^-1
+        e = _noise(Edge("chrom_single_freq", pulsars(EDGE4, 102, radio=True, single=(2,))), red=(-12.5, 3.0, 8), tm=True)
+        for i in range(e.b.n_psr):
+            e.dm(i, -12.3, 3.0, 8)
+        return e.curn(4).os(4, orfs=("hd",)).pfos().fp(n_freqs=3).rn(4)
+    R["chrom_single_freq"] = chrom_single_freq
+
+    def chrom_dm_only_rn():
+        # DM noise, no red noise: the red-noise likelihood leaves only the pulsar's own red noise out of P_a
+        e = _noise(Edge("chrom_dm_only_rn", pulsars(EDGE4, 103, radio=True)), tm=True)
+        for i in range(e.b.n_psr):
+            e.dm(i, -12.8, 2.0, 8)
+        return e.rn(4).curn(4)
+    R["chrom_dm_only_rn"] = chrom_dm_only_rn
+
+    def chrom_gw_modes():
+        # loud DM noise exactly on the GW basis frequencies
+        e = _noise(Edge("chrom_gw_modes", pulsars(EDGE4, 104, radio=True)), tm=True)
+        T = array_tspan(e.b)
+        for i in range(e.b.n_psr):
+            e.dm(i, -12.0, 3.0, 4, modes=np.arange(1, 5) / T)
+        return e.curn(4).os(4, orfs=("hd", "dipole")).pfos()
+    R["chrom_gw_modes"] = chrom_gw_modes
+
+    # 11. the red-noise likelihood's own: a pulsar spanning 3 days (a tiny T_a), and one Tspan for every pulsar
+    R["rn_short_span"] = lambda: _noise(Edge("rn_short_span", pulsars((5, 24, 65), 111, spans={1: (55000.0, 55003.0)})),
+                                        red=(-13.0, 3.0, 6)).rn(4)
+
+    def rn_tspan():
+        e = _noise(Edge("rn_tspan", pulsars(EDGE4, 112)), red=(-13.0, 3.0, 6), tm=True)
+        return e.rn(4, Tspan=1.5 * array_tspan(e.b))
+    R["rn_tspan"] = rn_tspan
+    R["rn_common"] = lambda: _noise(Edge("rn_common", pulsars(EDGE4, 113)), red=(-13.0, 3.0, 6), tm=True).rn(
+        4, log10_A_common=-13.5, gamma_common=3.0, components_common=6)
     return R
 
 

@@ -214,32 +214,6 @@ def test_ng15_dictionary_parses_as_before():
 
 
 # ------------------------------------------------------------------ P^-1 with chromatic blocks
-def _dense_pinv(b, i, F, tm):
-    """P_a^-1 F (long double) with the timing model marginalised: statics_reference's covariance plus the chromatic
-    terms (w w^T) ⊙ (F_s phi_s F_s^T)."""
-    LD = SR.LD
-    A = SR.covariance(b, i)
-    for c in b._chrom:
-        if c is not None and c["f"][i] is not None:
-            Fw = (c["weight"][i][:, None] * SR.basis(b.t_tdb[i], c["f"][i])).astype(LD)
-            A = A + (Fw * np.asarray(c["scale"][i], dtype=float).astype(LD) ** 2) @ Fw.T
-    L = SR.ld_cholesky(A)
-    M = SR.design(b, i, tm)
-    if M is None:
-        return SR.spd_solve(A, F.astype(LD), L)
-    if tm.get("dm") is not None:
-        t = b.t_tdb[i]
-        x = (t - 0.5 * (t.max() + t.min())) / (0.5 * (t.max() - t.min()))
-        w = (1400.0 / b.freq[i]) ** 2
-        M = np.concatenate([M, np.stack([w * x ** d for d in range(tm["dm"] + 1)], axis=1)], axis=1)
-    m = F.shape[1]
-    Y = SR.spd_solve(A, np.concatenate([F, M], axis=1).astype(LD), L)
-    PF, PM = Y[:, :m], Y[:, m:]
-    G = M.astype(LD).T @ PM
-    G = (G + G.T) / 2
-    return PF - PM @ SR.spd_solve(G, M.astype(LD).T @ PF)
-
-
 @pytest.mark.parametrize("case", ["all", "single_freq", "chrom_no_red", "dm_only"])
 def test_pinv_apply_with_chromatic_blocks(case):
     b = _batch(ntoas=(90, 70, 50), single=(1,) if case == "single_freq" else ())
@@ -252,11 +226,12 @@ def test_pinv_apply_with_chromatic_blocks(case):
         if case != "dm_only":
             b.set_chromatic_noise(i, -13.8, 3.5, idx=4.0, components=5)
         b.set_timing_model(i, poly=tm["poly"], dm=tm.get("dm"))
+    b._ref_chrom = {(slot, i): rec for i in range(b.n_psr) for slot, rec in ((0, (2.0, 1400.0)), (1, (4.0, 1400.0)))}
     for i in range(b.n_psr):
         F = SR.basis(b.t_tdb[i], np.arange(1, 4) / 3e8)
         d = b._white_variances("test")[i]
         got = b._pinv_apply(i, d, F)
-        ref = np.asarray(_dense_pinv(b, i, F, tm), dtype=float)
+        ref = np.asarray(SR.dense_pinv(b, i, F, tm=tm), dtype=float)
         scale = np.abs(ref).max(axis=0)
         assert np.all(np.abs(got - ref) <= 1e-8 * scale), (case, i, float(np.max(np.abs(got - ref) / scale)))
 

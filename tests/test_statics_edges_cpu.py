@@ -35,6 +35,7 @@ KNOWN = {
     ("corners_k16_hd", "hd"): (("hd lnL", "hd ldet"), "eigen", "gamma = 7, K = 16, N = 64"),
     ("orf_rank2", "hd"): (("hd lnL",), "eigen", "rank-2 ORF"),
     ("rankdef", "curn"): (("curn lnL", "curn ldet"), "eigen", "n_a = 5, 6, 7 < 2K = 32"),
+    ("chrom_dm_only_rn", "curn"): (("curn lnL", "curn ldet"), "eigen", "loud DM noise, gamma = 7 at log10_A = -11"),
     ("red_gw_modes", "curn"): (("curn lnL", "curn ldet"), "woodbury", "loud red noise on the GW frequencies"),
     ("red_loud", "curn"): (("curn lnL", "curn ldet"), "woodbury", "loud steep red noise, 30 components"),
     ("red_loud_hd", "curn"): (("curn lnL", "curn ldet"), "woodbury", "loud steep red noise, K = 1"),
@@ -98,11 +99,12 @@ def fe_of_statics(pe, amps):
 
 
 # ------------------------------------------------------------------ cases
-def _kappa(e, common=None):
-    """The largest kappa of the pulsars' Woodbury matrices S and of their ECORR Sherman-Morrison steps
-    (1 + e^2 sum_bucket 1/sigma^2, the cancellation of N^-1 V within a bucket)."""
+def _kappa(e, common=None, own_red=True):
+    """The largest kappa of the pulsars' Woodbury matrices S (chromatic blocks included; the red noise left out with
+    ``own_red`` False) and of their ECORR Sherman-Morrison steps (1 + e^2 sum_bucket 1/sigma^2, the cancellation of
+    N^-1 V within a bucket)."""
     b = e.b
-    k = max(SR.woodbury_cond(b, i, common, e.tm[i]) for i in range(b.n_psr))
+    k = max(SR.woodbury_cond(b, i, common, e.tm[i], own_red) for i in range(b.n_psr))
     if b._ecorr is not None:
         for i in range(b.n_psr):
             bucket, ec = b._ecorr[i]
